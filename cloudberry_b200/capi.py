@@ -29,6 +29,11 @@ class CbgpuVisimapEntry(C.Structure):
     _fields_ = [("first_row_num", C.c_int64), ("data", C.c_void_p), ("len", C.c_int32)]
 
 
+class CbgpuPairs(C.Structure):
+    """cbgpu_pairs: (outer, inner) row ids of a pair probe, two device arrays (cbgpu_pairs_free)"""
+    _fields_ = [("npairs", C.c_int64), ("outer_idx", C.c_void_p), ("inner_idx", C.c_void_p)]
+
+
 class CbAggStateDatum(C.Structure):
     _fields_ = [("n", C.c_int64), ("lo", C.c_int64), ("hi", C.c_int64)]
 
@@ -323,6 +328,11 @@ def gpu():
             "cbgpu_ht_nrows": (i64, [vp]),
             "cbgpu_ht_has_duplicates": (C.c_int, [vp]),
             "cbgpu_ht_probe_pairs": (C.c_int, [vp, vp, vp, C.POINTER(i32), i32, vp, i64, vp]),
+            "cbgpu_ht_probe_pairs_outer": (C.c_int, [vp, vp, vp, C.POINTER(i32), i32, i32, i32, vp]),
+            "cbgpu_ht_build_batched": (C.c_int, [vp, vp, C.POINTER(i32), i32, i32, C.POINTER(vp)]),
+            "cbgpu_ht_nbatch": (C.c_int, [vp]),
+            "cbgpu_ht_load_batch": (C.c_int, [vp, i32]),
+            "cbgpu_ht_probe_pairs_batched": (C.c_int, [vp, vp, vp, C.POINTER(i32), i32, i32, i32, vp, vp, vp, C.POINTER(i64)]),
             "cbgpu_pairs_free": (None, [vp]),
             "cbgpu_merge_sorted_runs": (C.c_int, [vp, vp, C.POINTER(i32), C.POINTER(i32), C.POINTER(i32), i32, i32, C.POINTER(vp),
                                                   C.POINTER(i32)]),

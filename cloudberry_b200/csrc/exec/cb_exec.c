@@ -1004,6 +1004,15 @@ inner_out_exprs(CbEState *es, CbStream *s, NodePriv *hp, int src, int nullable, 
 	return CBGPU_OK;
 }
 
+/* CHECK_FOR_INTERRUPTS between the batches of a pair join, as run_pipeline polls between its passes */
+static int
+hj_interrupted(void *arg)
+{
+	CbEState   *es = (CbEState *) arg;
+
+	return es->es_interrupt_pending && es->es_interrupt_pending(es);
+}
+
 static int
 open_hashjoin(CbPlanState *ps, CbStream **out)
 {
@@ -1058,8 +1067,6 @@ open_hashjoin(CbPlanState *ps, CbStream **out)
 		NodePriv   *me = np(ps);
 		int			c;
 
-		if (cbgpu_ht_nbatch(hp->ht) > 1)
-			return es_fail(es, CBGPU_ERR_UNSUPPORTED, "multi-batch hash join with duplicate build keys is not implemented on the GPU path (raise the operator memory)");
 		/* append the key expressions as extra output columns so the probe can read them */
 		for (int k = 0; k < hj->nhashkeys; k++)
 		{
@@ -1076,7 +1083,20 @@ open_hashjoin(CbPlanState *ps, CbStream **out)
 		if (me->owned.npairs >= 8)
 			return es_fail(es, CBGPU_ERR_UNSUPPORTED, "too many N:M joins under one node");
 		pairs = &me->owned.pairs[me->owned.npairs++];
-		GPU(es, cbgpu_ht_probe_pairs_outer(es->es_ctx, hp->ht, orel, keycols, hj->nhashkeys, fill_outer, fill_inner, pairs));
+		if (cbgpu_ht_nbatch(hp->ht) > 1)
+		{
+			/* a build side split into batches: one pass per batch, each probed by its own outer rows; the pairs of all passes
+			 * come back as one list, so nothing downstream knows */
+			int64_t		passes = 0;
+			int			rc = cbgpu_ht_probe_pairs_batched(es->es_ctx, hp->ht, orel, keycols, hj->nhashkeys, fill_outer, fill_inner,
+														  hj_interrupted, es, pairs, &passes);
+
+			es->es_hashjoin_batches_run += passes;
+			if (rc != CBGPU_OK)
+				return es_fail(es, rc, "%s", cbgpu_last_error(es->es_ctx));
+		}
+		else
+			GPU(es, cbgpu_ht_probe_pairs_outer(es->es_ctx, hp->ht, orel, keycols, hj->nhashkeys, fill_outer, fill_inner, pairs));
 		s2 = stream_new(me);
 		TRY(stream_over_rel(es, s2, orel, shape, nouter));
 		if (fill_inner)

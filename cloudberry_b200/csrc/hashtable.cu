@@ -452,6 +452,27 @@ struct ProbeParams
 	uint32_t   *out_inner;
 };
 
+/* an outer row's key hash (ht_row_hash over the probe side's columns) and its batch: the bits ht_in_batch tests, and batch 0
+ * for a NULL key, which never matches (the N:1 probe and the reference put such rows there too).  The batch partition and the
+ * pair probe both decide a row's batch here, so that a row is probed, or NULL-extended, in exactly one pass. */
+__device__ __forceinline__ int32_t
+ht_probe_row_batch(const ProbeParams &p, uint32_t row, int64_t *key, uint32_t *hash, bool *keynull)
+{
+	uint32_t	h = 0;
+	bool		isnull = false;
+
+	for (int k = 0; k < p.ht.nkeys; k++)
+	{
+		if (p.onulls[k] && p.onulls[k][row])
+			isnull = true;
+		key[k] = cb_load_widen(p.okey[k], p.otype[k], row);
+		h = pg_hash_combine(h, jh_hash_datum(p.otype[k], key[k], p.odict[k]), false);
+	}
+	*hash = h;
+	*keynull = isnull;
+	return (p.ht.nbatch <= 1 || isnull) ? 0 : (int32_t) (h >> p.ht.batch_shift);
+}
+
 template <bool WRITE>
 __global__ void __launch_bounds__(256)
 k_ht_probe_pairs(ProbeParams p)
@@ -462,19 +483,13 @@ k_ht_probe_pairs(ProbeParams p)
 	for (; i < p.n; i += stride)
 	{
 		uint32_t	row = p.sel ? p.sel[i] : (uint32_t) i;
-		uint32_t	h = 0;
+		uint32_t	h;
 		int64_t		key[CBP_MAX_KEYS];
-		bool		isnull = false;
+		bool		isnull;
+		const bool	mine = ht_probe_row_batch(p, row, key, &h, &isnull) == p.ht.batch_id || p.ht.nbatch <= 1;
 		unsigned long long cnt = 0;
 		unsigned long long base = WRITE ? p.counts[i] : 0;
 
-		for (int k = 0; k < p.ht.nkeys; k++)
-		{
-			if (p.onulls[k] && p.onulls[k][row])
-				isnull = true;
-			key[k] = cb_load_widen(p.okey[k], p.otype[k], row);
-			h = pg_hash_combine(h, jh_hash_datum(p.otype[k], key[k], p.odict[k]), false);
-		}
 		if (!isnull && p.ht.bloom)
 		{
 			uint32_t	w;
@@ -485,7 +500,7 @@ k_ht_probe_pairs(ProbeParams p)
 		}
 		if (!isnull && p.ht.keyslot && !ht_key_in_domain(p.ht.keyslot, key[0]))
 			isnull = true;			/* outside the build side's key domain: no partner */
-		if (!isnull && !ht_in_batch(p.ht.nbatch, p.ht.batch_shift, p.ht.batch_id, h))
+		if (!isnull && !mine)
 			isnull = true;			/* multi-batch join: this row belongs to another pass */
 		if (!isnull)
 		{
@@ -520,7 +535,7 @@ k_ht_probe_pairs(ProbeParams p)
 				pos = (pos + 1) & p.ht.mask;
 			}
 		}
-		if (p.left && cnt == 0 && ht_in_batch(p.ht.nbatch, p.ht.batch_shift, p.ht.batch_id, h))
+		if (p.left && cnt == 0 && mine)
 		{
 			/* no partner (or a NULL key, which never has one): the outer row survives with a NULL inner side */
 			if (WRITE)
@@ -621,6 +636,94 @@ k_ht_unmatched_write(ProbeParams p)
 		}
 }
 
+/* ---------------------------------------------------------------------------------------------
+ * The probe side of a multi-batch pair join, partitioned by batch once (the reference writes each outer tuple to its batch's
+ * file instead: ExecHashJoinSaveTuple, nodeHashjoin.c): a stable counting sort of the outer row ids into nbatch runs.  Each
+ * CTA owns a contiguous chunk of rows.  k_ht_partition_count reads the key columns, keeps every row's batch and counts its
+ * chunk's rows per batch; an exclusive scan over the [batch][CTA] counts gives each (batch, CTA) its first position; then
+ * k_ht_partition_write places the rows tile by tile, the warps of a tile in order, so each run lists its rows in relation
+ * order and the pair list's probe-row order is the same on every run.
+ * --------------------------------------------------------------------------------------------- */
+#define HT_PART_THREADS 256
+
+__global__ void __launch_bounds__(HT_PART_THREADS)
+k_ht_partition_count(ProbeParams p, int64_t chunk, uint16_t *rowbatch, unsigned long long *hist)
+{
+	extern __shared__ uint32_t cnt[];	/* [nbatch] */
+	const int64_t lo = (int64_t) blockIdx.x * chunk;
+	const int64_t hi = lo + chunk < p.n ? lo + chunk : p.n;
+
+	for (int b = threadIdx.x; b < p.ht.nbatch; b += blockDim.x)
+		cnt[b] = 0;
+	__syncthreads();
+	for (int64_t i0 = lo; i0 < hi; i0 += blockDim.x)
+	{
+		const int64_t i = i0 + threadIdx.x;
+		int32_t		b = -1;
+
+		if (i < hi)
+		{
+			int64_t		key[CBP_MAX_KEYS];
+			uint32_t	h;
+			bool		isnull;
+
+			b = ht_probe_row_batch(p, (uint32_t) i, key, &h, &isnull);
+			rowbatch[i] = (uint16_t) b;
+		}
+		/* one shared-memory atomic per batch and warp: with a skewed key every row lands in the same counter */
+		const unsigned peers = __match_any_sync(0xffffffffu, b);
+
+		if (b >= 0 && (int) (threadIdx.x & 31) == __ffs(peers) - 1)
+			atomicAdd(cnt + b, (uint32_t) __popc(peers));
+	}
+	__syncthreads();
+	for (int b = threadIdx.x; b < p.ht.nbatch; b += blockDim.x)
+		hist[(int64_t) b * gridDim.x + blockIdx.x] = cnt[b];
+}
+
+__global__ void __launch_bounds__(HT_PART_THREADS)
+k_ht_partition_write(int64_t n, int32_t nbatch, int64_t chunk, const uint16_t *rowbatch, const unsigned long long *start,
+					 unsigned long long *offsets, uint32_t *rows)
+{
+	extern __shared__ uint32_t cur[];	/* [nbatch] where the chunk's next row of each batch goes (row ids are 32 bits) */
+	const int64_t lo = (int64_t) blockIdx.x * chunk;
+	const int64_t hi = lo + chunk < n ? lo + chunk : n;
+	const int	lane = threadIdx.x & 31,
+				warp = threadIdx.x >> 5;
+
+	for (int b = threadIdx.x; b < nbatch; b += blockDim.x)
+		cur[b] = (uint32_t) start[(int64_t) b * gridDim.x + blockIdx.x];
+	if (blockIdx.x == 0)
+		for (int b = threadIdx.x; b <= nbatch; b += blockDim.x)
+			offsets[b] = start[(int64_t) b * gridDim.x];	/* b == nbatch: the scan's total, n */
+	__syncthreads();
+	for (int64_t i0 = lo; i0 < hi; i0 += blockDim.x)
+	{
+		const int64_t i = i0 + threadIdx.x;
+		const int32_t b = i < hi ? (int32_t) rowbatch[i] : -1;
+		const unsigned peers = __match_any_sync(0xffffffffu, b);
+		const uint32_t rank = __popc(peers & ((1u << lane) - 1));
+
+		/* warp w's rows follow those of warps 0 .. w-1 of the same tile */
+		for (int w = 0; w < (int) (blockDim.x >> 5); w++)
+		{
+			if (warp == w)
+			{
+				const uint32_t at = b >= 0 ? cur[b] : 0;
+
+				__syncwarp();
+				if (b >= 0)
+				{
+					rows[at + rank] = (uint32_t) i;
+					if (rank == 0)
+						cur[b] = at + (uint32_t) __popc(peers);
+				}
+			}
+			__syncthreads();
+		}
+	}
+}
+
 static int	ht_probe_pairs(cbgpu_ctx *ctx, const cbgpu_hashtable *ht, cbgpu_rel *outer, const int32_t *keycols, int32_t nkeys,
 						   const uint32_t *sel, int64_t nsel, int left, int fill_inner, cbgpu_pairs *out);
 
@@ -645,6 +748,28 @@ cbgpu_ht_probe_pairs_left(cbgpu_ctx *ctx, const cbgpu_hashtable *ht, cbgpu_rel *
 	return ht_probe_pairs(ctx, ht, outer, keycols, nkeys, NULL, 0, 1, 0, out);
 }
 
+/* the probe side's key columns of a pair probe */
+static int
+probe_params(cbgpu_ctx *ctx, const cbgpu_hashtable *ht, cbgpu_rel *outer, const int32_t *keycols, int32_t nkeys, ProbeParams *p)
+{
+	if (nkeys != ht->d.nkeys)
+		return cb_fail(ctx, CBGPU_ERR_INVALID, "cbgpu_ht_probe_pairs: key count mismatch%s %lld", "", nkeys);
+	memset(p, 0, sizeof(*p));
+	p->ht = ht->d;
+	for (int k = 0; k < nkeys; k++)
+	{
+		int			c = keycols[k];
+
+		if (c < 0 || c >= outer->ncols)
+			return cb_fail(ctx, CBGPU_ERR_INVALID, "cbgpu_ht_probe_pairs: bad key column%s %lld", "", c);
+		p->okey[k] = outer->data[c];
+		p->onulls[k] = outer->nulls[c];
+		p->odict[k] = outer->dict_hash[c];
+		p->otype[k] = outer->types[c];
+	}
+	return CBGPU_OK;
+}
+
 static int
 ht_probe_pairs(cbgpu_ctx *ctx, const cbgpu_hashtable *ht, cbgpu_rel *outer, const int32_t *keycols, int32_t nkeys,
 			   const uint32_t *sel, int64_t nsel, int left, int fill_inner, cbgpu_pairs *out)
@@ -653,31 +778,21 @@ ht_probe_pairs(cbgpu_ctx *ctx, const cbgpu_hashtable *ht, cbgpu_rel *outer, cons
 	int64_t		n = sel ? nsel : outer->nrows;
 	unsigned long long total = 0;
 	const int64_t ninner = fill_inner ? ht->inner->nrows : 0;
+	int			rc;
 
 	memset(out, 0, sizeof(*out));
-	if (nkeys != ht->d.nkeys)
-		return cb_fail(ctx, CBGPU_ERR_INVALID, "cbgpu_ht_probe_pairs: key count mismatch%s %lld", "", nkeys);
-	memset(&p, 0, sizeof(p));
-	p.ht = ht->d;
-	for (int k = 0; k < nkeys; k++)
-	{
-		int			c = keycols[k];
-
-		if (c < 0 || c >= outer->ncols)
-			return cb_fail(ctx, CBGPU_ERR_INVALID, "cbgpu_ht_probe_pairs: bad key column%s %lld", "", c);
-		p.okey[k] = outer->data[c];
-		p.onulls[k] = outer->nulls[c];
-		p.odict[k] = outer->dict_hash[c];
-		p.otype[k] = outer->types[c];
-	}
+	/* one pass sees the resident batch only: the probe rows of every other batch would be missing from the result */
+	if (ht->d.nbatch > 1)
+		return cb_fail(ctx, CBGPU_ERR_INVALID, "%sa table of %lld batches is probed for pairs by cbgpu_ht_probe_pairs_batched", "",
+					   ht->d.nbatch);
+	if ((rc = probe_params(ctx, ht, outer, keycols, nkeys, &p)) != CBGPU_OK)
+		return rc;
 	p.sel = sel;
 	p.n = n;
 	p.left = left;
 	p.ninner = ninner;
 	if (n + ninner == 0)
 		return CBGPU_OK;
-	if (fill_inner && ht->d.nbatch > 1)
-		return cb_fail(ctx, CBGPU_ERR_UNSUPPORTED, "RIGHT / FULL join over a multi-batch table is not implemented%s", "");
 	CB_CUDA(ctx, cudaMallocAsync(&p.counts, (size_t) (n + ninner + 1) * sizeof(unsigned long long), ctx->stream));
 	if (ninner)
 	{
@@ -734,6 +849,216 @@ ht_probe_pairs(cbgpu_ctx *ctx, const cbgpu_hashtable *ht, cbgpu_rel *outer, cons
 		CB_CUDA(ctx, cudaFreeAsync(p.matched, ctx->stream));
 	CB_CUDA(ctx, cudaFreeAsync(p.counts, ctx->stream));
 	return CBGPU_OK;
+}
+
+/* the device and host buffers of a batched pair probe: freed by cbgpu_ht_probe_pairs_batched whatever the outcome */
+struct BatchedProbe
+{
+	uint16_t   *rowbatch;		/* [n] each outer row's batch                                              */
+	unsigned long long *hist;	/* [nbatch][partition CTAs] row counts, then their exclusive scan          */
+	unsigned long long *d_offsets;	/* [nbatch + 1] where each batch's run starts in rows                  */
+	unsigned long long *h_offsets;
+	uint32_t   *rows;			/* [n] outer row ids grouped by batch                                       */
+	unsigned long long *counts;	/* match counts of one run (or of the build rows), then their scan          */
+	uint8_t    *matched;		/* RIGHT / FULL: [inner rows], kept across all passes                       */
+	uint32_t   *grow[2];		/* the output's next, larger arrays while they are being filled             */
+	int64_t		cap;			/* pairs the output arrays hold                                             */
+};
+
+/* room for `need` pairs in out, keeping the out->npairs written so far (capacity doubles: the copies stay linear) */
+static int
+pairs_reserve(cbgpu_ctx *ctx, BatchedProbe *b, cbgpu_pairs *out, int64_t need)
+{
+	const int64_t cap = b->cap * 2 > need ? b->cap * 2 : need;
+
+	if (need <= b->cap)
+		return CBGPU_OK;
+	CB_CUDA(ctx, cudaMalloc(&b->grow[0], (size_t) cap * sizeof(uint32_t)));
+	CB_CUDA(ctx, cudaMalloc(&b->grow[1], (size_t) cap * sizeof(uint32_t)));
+	if (out->npairs)
+	{
+		CB_CUDA(ctx, cudaMemcpyAsync(b->grow[0], out->outer_idx, (size_t) out->npairs * sizeof(uint32_t), cudaMemcpyDeviceToDevice, ctx->stream));
+		CB_CUDA(ctx, cudaMemcpyAsync(b->grow[1], out->inner_idx, (size_t) out->npairs * sizeof(uint32_t), cudaMemcpyDeviceToDevice, ctx->stream));
+		CB_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+	}
+	if (out->outer_idx)
+		cudaFree(out->outer_idx);
+	if (out->inner_idx)
+		cudaFree(out->inner_idx);
+	out->outer_idx = b->grow[0];
+	out->inner_idx = b->grow[1];
+	b->grow[0] = b->grow[1] = NULL;
+	b->cap = cap;
+	return CBGPU_OK;
+}
+
+/* the pairs whose counts p.counts[0 .. nc) holds, appended to out: scan, one read-back, room, then `write` */
+static int
+pairs_append(cbgpu_ctx *ctx, BatchedProbe *b, ProbeParams *p, int64_t nc, cbgpu_pairs *out, bool *any)
+{
+	unsigned long long t = 0;
+
+	k_exclusive_scan_u64<<<1, 1024, 0, ctx->stream>>>(p->counts, nc);
+	CB_LAUNCHED(ctx, "k_exclusive_scan_u64");
+	CB_CUDA(ctx, cudaMemcpyAsync(&t, p->counts + nc, sizeof(t), cudaMemcpyDeviceToHost, ctx->stream));
+	CB_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+	if ((unsigned long long) out->npairs + t > 0xFFFFFFF0ull)
+		return cb_fail(ctx, CBGPU_ERR_UNSUPPORTED, "join result of %s%lld pairs exceeds the GPU path's 32-bit row ids", "",
+					   (long long) (out->npairs + t));
+	*any = t > 0;
+	if (t == 0)
+		return CBGPU_OK;
+	int			rc = pairs_reserve(ctx, b, out, out->npairs + (int64_t) t);
+
+	if (rc != CBGPU_OK)
+		return rc;
+	p->out_outer = out->outer_idx + out->npairs;
+	p->out_inner = out->inner_idx + out->npairs;
+	out->npairs += (int64_t) t;
+	return CBGPU_OK;
+}
+
+static int
+ht_probe_batched(cbgpu_ctx *ctx, cbgpu_hashtable *ht, ProbeParams p, int fill_inner, int (*interrupted)(void *arg), void *arg,
+				 BatchedProbe *b, cbgpu_pairs *out, int64_t *passes)
+{
+	const int32_t nbatch = ht->d.nbatch;
+	const int64_t n = p.n;
+	const int64_t ninner = fill_inner ? ht->inner->nrows : 0;
+	int64_t		maxrun = 0;
+	bool		any;
+	int			rc;
+
+	CB_CUDA(ctx, cudaSetDevice(ctx->device));
+	b->h_offsets = (unsigned long long *) calloc((size_t) nbatch + 1, sizeof(unsigned long long));
+	if (!b->h_offsets)
+		return cb_fail(ctx, CBGPU_ERR_NOMEM, "host memory for %s%lld batch offsets", "", nbatch);
+	if (n > 0)
+	{
+		/* at most 2^18 [batch][CTA] counts: the scan over them runs on one CTA */
+		int64_t		grid = (int64_t) ctx->sm_count * 2,
+					chunk;
+		const size_t shmem = (size_t) nbatch * sizeof(uint32_t);
+
+		if (grid > (1 << 18) / nbatch)
+			grid = (1 << 18) / nbatch;
+		if (grid > (n + HT_PART_THREADS - 1) / HT_PART_THREADS)
+			grid = (n + HT_PART_THREADS - 1) / HT_PART_THREADS;
+		chunk = (n + grid - 1) / grid;
+		CB_CUDA(ctx, cudaMallocAsync(&b->rowbatch, (size_t) n * sizeof(uint16_t), ctx->stream));
+		CB_CUDA(ctx, cudaMallocAsync(&b->hist, ((size_t) nbatch * grid + 1) * sizeof(unsigned long long), ctx->stream));
+		CB_CUDA(ctx, cudaMallocAsync(&b->d_offsets, ((size_t) nbatch + 1) * sizeof(unsigned long long), ctx->stream));
+		CB_CUDA(ctx, cudaMallocAsync(&b->rows, (size_t) n * sizeof(uint32_t), ctx->stream));
+		k_ht_partition_count<<<(int) grid, HT_PART_THREADS, shmem, ctx->stream>>>(p, chunk, b->rowbatch, b->hist);
+		CB_LAUNCHED(ctx, "k_ht_partition_count");
+		k_exclusive_scan_u64<<<1, 1024, 0, ctx->stream>>>(b->hist, nbatch * grid);
+		CB_LAUNCHED(ctx, "k_exclusive_scan_u64");
+		k_ht_partition_write<<<(int) grid, HT_PART_THREADS, shmem, ctx->stream>>>(n, nbatch, chunk, b->rowbatch, b->hist, b->d_offsets,
+																				   b->rows);
+		CB_LAUNCHED(ctx, "k_ht_partition_write");
+		CB_CUDA(ctx, cudaMemcpyAsync(b->h_offsets, b->d_offsets, ((size_t) nbatch + 1) * sizeof(unsigned long long),
+									 cudaMemcpyDeviceToHost, ctx->stream));
+		CB_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+		for (int32_t k = 0; k < nbatch; k++)
+			if ((int64_t) (b->h_offsets[k + 1] - b->h_offsets[k]) > maxrun)
+				maxrun = (int64_t) (b->h_offsets[k + 1] - b->h_offsets[k]);
+	}
+	CB_CUDA(ctx, cudaMallocAsync(&b->counts, (size_t) ((maxrun > ninner ? maxrun : ninner) + 1) * sizeof(unsigned long long), ctx->stream));
+	p.counts = b->counts;
+	if (ninner)
+	{
+		CB_CUDA(ctx, cudaMallocAsync(&b->matched, (size_t) ninner, ctx->stream));
+		CB_CUDA(ctx, cudaMemsetAsync(b->matched, 0, (size_t) ninner, ctx->stream));
+		p.matched = b->matched;
+	}
+	/* HJ_NEED_NEW_BATCH (nodeHashjoin.c:709-738): each batch resident in turn, probed by its own run of outer rows */
+	for (int32_t batch = 0; batch < nbatch; batch++)
+	{
+		const int64_t m = (int64_t) (b->h_offsets[batch + 1] - b->h_offsets[batch]);
+		int			blocks = (int) ((m + 255) / 256);
+
+		if (interrupted && interrupted(arg))
+			return cb_fail(ctx, CBGPU_ERR_INTERRUPTED, "canceling statement due to user request%s", "");
+		if ((rc = cbgpu_ht_load_batch(ht, batch)) != CBGPU_OK)
+			return rc;
+		(*passes)++;
+		if (m == 0)
+			continue;
+		if (blocks > ctx->sm_count * 8)
+			blocks = ctx->sm_count * 8;
+		p.ht = ht->d;
+		p.sel = b->rows + b->h_offsets[batch];
+		p.n = m;
+		k_ht_probe_pairs<false><<<blocks, 256, 0, ctx->stream>>>(p);
+		CB_LAUNCHED(ctx, "k_ht_probe_pairs<count>");
+		if ((rc = pairs_append(ctx, b, &p, m, out, &any)) != CBGPU_OK)
+			return rc;
+		if (any)
+		{
+			k_ht_probe_pairs<true><<<blocks, 256, 0, ctx->stream>>>(p);
+			CB_LAUNCHED(ctx, "k_ht_probe_pairs<write>");
+		}
+	}
+	if (ninner)
+	{
+		/* every pass has marked its matches: the build rows left unmatched come back once, behind all matched pairs */
+		int			iblocks = (int) ((ninner + 255) / 256);
+
+		if (iblocks > ctx->sm_count * 8)
+			iblocks = ctx->sm_count * 8;
+		p.sel = NULL;
+		p.n = 0;
+		p.ninner = ninner;
+		k_ht_unmatched_count<<<iblocks, 256, 0, ctx->stream>>>(p);
+		CB_LAUNCHED(ctx, "k_ht_unmatched_count");
+		if ((rc = pairs_append(ctx, b, &p, ninner, out, &any)) != CBGPU_OK)
+			return rc;
+		if (any)
+		{
+			k_ht_unmatched_write<<<iblocks, 256, 0, ctx->stream>>>(p);
+			CB_LAUNCHED(ctx, "k_ht_unmatched_write");
+		}
+	}
+	return CBGPU_OK;
+}
+
+extern "C" int
+cbgpu_ht_probe_pairs_batched(cbgpu_ctx *ctx, cbgpu_hashtable *ht, cbgpu_rel *outer, const int32_t *keycols, int32_t nkeys,
+							 int32_t fill_outer, int32_t fill_inner, int (*interrupted)(void *arg), void *arg, cbgpu_pairs *out,
+							 int64_t *passes)
+{
+	BatchedProbe b;
+	ProbeParams p;
+	int64_t		npasses = 0;
+	int			rc;
+
+	if (passes)
+		*passes = 0;
+	if (ht->d.nbatch <= 1)
+		return ht_probe_pairs(ctx, ht, outer, keycols, nkeys, NULL, 0, fill_outer != 0, fill_inner != 0, out);
+	memset(out, 0, sizeof(*out));
+	if ((rc = probe_params(ctx, ht, outer, keycols, nkeys, &p)) != CBGPU_OK)
+		return rc;
+	p.n = outer->nrows;
+	p.left = fill_outer != 0;
+	memset(&b, 0, sizeof(b));
+	rc = ht_probe_batched(ctx, ht, p, fill_inner != 0, interrupted, arg, &b, out, &npasses);
+	if (passes)
+		*passes = npasses;
+	{
+		void	   *dev[] = {b.rowbatch, b.hist, b.d_offsets, b.rows, b.counts, b.matched};
+
+		for (size_t k = 0; k < sizeof(dev) / sizeof(dev[0]); k++)
+			if (dev[k])
+				cudaFreeAsync(dev[k], ctx->stream);
+	}
+	for (int k = 0; k < 2; k++)
+		if (b.grow[k])
+			cudaFree(b.grow[k]);
+	free(b.h_offsets);
+	if (rc != CBGPU_OK)
+		cbgpu_pairs_free(out);
+	return rc;
 }
 
 extern "C" void

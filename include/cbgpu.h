@@ -324,6 +324,18 @@ int			cbgpu_ht_probe_pairs_left(cbgpu_ctx *ctx, const cbgpu_hashtable *ht, cbgpu
  * FULL: ExecScanHashTableForUnmatched nodeHash.c:2360, HJ_FILL_INNER_TUPLES nodeHashjoin.c:676-706) */
 int			cbgpu_ht_probe_pairs_outer(cbgpu_ctx *ctx, const cbgpu_hashtable *ht, cbgpu_rel *outer, const int32_t *keycols,
 									   int32_t nkeys, int32_t fill_outer, int32_t fill_inner, cbgpu_pairs *out);
+/* The three calls above probe the resident batch only, so they refuse a table of several batches (CBGPU_ERR_INVALID).
+ * This one runs the whole join over such a table (ExecHashJoinImpl's HJ_NEED_NEW_BATCH loop, nodeHashjoin.c:709-738): every
+ * row of `outer` is assigned to its key's batch once, then each batch is loaded in turn (0 .. nbatch - 1) and probed by its
+ * own rows, and for fill_inner the build rows no batch matched come last.  fill_outer / fill_inner as in
+ * cbgpu_ht_probe_pairs_outer; a NULL-keyed probe row belongs to batch 0.  Within one batch pairs are in outer-row order,
+ * so the outer row ids come in the same order on every call (a row's partners in the table's slot order).  `interrupted` (may be NULL) is polled before each batch: nonzero stops the call with
+ * CBGPU_ERR_INTERRUPTED.  *passes (may be NULL) = batches loaded and probed, also when the call fails.  On return the
+ * table holds the last batch it loaded (nbatch - 1 after a success).  A one-batch table takes cbgpu_ht_probe_pairs_outer's
+ * path with *passes = 0.  On failure *out is empty and nothing stays allocated. */
+int			cbgpu_ht_probe_pairs_batched(cbgpu_ctx *ctx, cbgpu_hashtable *ht, cbgpu_rel *outer, const int32_t *keycols,
+										 int32_t nkeys, int32_t fill_outer, int32_t fill_inner, int (*interrupted) (void *arg),
+										 void *arg, cbgpu_pairs *out, int64_t *passes);
 void		cbgpu_pairs_free(cbgpu_pairs *p);
 int			cbgpu_read_u32(cbgpu_ctx *ctx, const uint32_t *dev, int64_t n, uint32_t *host);
 /* small device scratch (sink row counters, index vectors): zero-filled allocation, read-back, free */
