@@ -50,12 +50,11 @@ struct cbgpu_ctx
 								 * synchronising read-back fetches the status word too, so the check
 								 * after it costs no second round trip                                 */
 	/* environment knobs (DESIGN.md 9), read ONCE when the context is created - not per launch */
-	bool		opt_debug, opt_no_early_filter, opt_no_keyslot, opt_no_fuse0, opt_no_spec0, opt_no_smem_ht, opt_l2_direct, opt_no_prefilter, opt_prefilter_tma, opt_pf_spec, opt_pf_occ6;
+	bool		opt_debug, opt_pf_spec;
 	int			opt_bloom_div;
-	int			opt_htb_u;		/* rows a hash-build thread keeps in flight (CBGPU_HTB_U: 1, 2, 4)          */
 	/* host-side scratch of the launch path (decompiled programs, kernel parameter blocks: too large for the
 	 * stack), owned by the context so that two contexts on two threads never share any: slot -> malloc'ed block */
-#define CB_SCRATCH_SLOTS 8
+#define CB_SCRATCH_SLOTS 7
 	void	   *scratch[CB_SCRATCH_SLOTS];
 	size_t		scratch_bytes[CB_SCRATCH_SLOTS];
 	/* scan-level runtime filter decisions, remembered per (build relation, rows, key column): the sample that

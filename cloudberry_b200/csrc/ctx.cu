@@ -56,19 +56,9 @@ cbgpu_ctx_create(int device, cbgpu_ctx **out)
 	CB_CUDA(ctx, cudaMallocHost(&ctx->agg_snap, sizeof(AggSnap)));
 	memset(ctx->agg_snap, 0, sizeof(AggSnap));
 	ctx->opt_debug = getenv("CBGPU_DEBUG") != NULL;
-	ctx->opt_no_early_filter = getenv("CBGPU_NO_EARLY_FILTER") != NULL;
-	ctx->opt_no_keyslot = getenv("CBGPU_NO_KEYSLOT") != NULL;
-	ctx->opt_no_fuse0 = getenv("CBGPU_NO_FUSE0") != NULL;
-	ctx->opt_no_spec0 = getenv("CBGPU_SPEC0") == NULL;	/* loading probe 0's keys with the qual columns was slower on Q3: off unless asked for */
-	ctx->opt_no_smem_ht = getenv("CBGPU_NO_SMEM_HT") != NULL;
-	ctx->opt_no_prefilter = getenv("CBGPU_NO_PREFILTER") != NULL;
-	ctx->opt_prefilter_tma = getenv("CBGPU_PREFILTER_TMA") != NULL;
 	ctx->opt_pf_spec = getenv("CBGPU_PF_SPEC") != NULL;
 	ctx->opt_pf_keep_div = getenv("CBGPU_PREFILTER_KEEP_DIV") && atoi(getenv("CBGPU_PREFILTER_KEEP_DIV")) > 0 ? atoi(getenv("CBGPU_PREFILTER_KEEP_DIV")) : 12;
-	ctx->opt_pf_occ6 = getenv("CBGPU_PF_OCC6") != NULL;
 	ctx->opt_pf_min_rows = getenv("CBGPU_PREFILTER_MIN_ROWS") ? atoll(getenv("CBGPU_PREFILTER_MIN_ROWS")) : ((int64_t) 16 << 20);
-	ctx->opt_l2_direct = getenv("CBGPU_L2_DIRECT") != NULL;
-	ctx->opt_htb_u = getenv("CBGPU_HTB_U") && atoi(getenv("CBGPU_HTB_U")) > 0 ? atoi(getenv("CBGPU_HTB_U")) : 1;
 	ctx->opt_bloom_div = getenv("CBGPU_BLOOM_DIV") && atoi(getenv("CBGPU_BLOOM_DIV")) > 0 ? atoi(getenv("CBGPU_BLOOM_DIV")) : 2;
 	/* L2 is 50 MB on H100: flush buffer comfortably larger */
 	ctx->flush_bytes = (size_t) 512 << 20;

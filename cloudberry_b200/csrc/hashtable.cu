@@ -62,9 +62,6 @@ k_ht_clear(unsigned long long *slots, size_t n)
 		slots[i] = HT_EMPTY;
 }
 
-/* U rows of a thread in flight: their key loads, then their filter words, then their first slots are issued back to back
- * (a row's chain key -> filter word -> slot -> compare-and-swap is four dependent memory operations, the table rarely fits L2) */
-template <int HTB_U>
 __global__ void __launch_bounds__(256)
 k_ht_build(BuildParams p)
 {
@@ -73,69 +70,53 @@ k_ht_build(BuildParams p)
 	bool		dup = false;
 	bool		outside = false;
 
-	for (int64_t i0 = (int64_t) blockIdx.x * blockDim.x + threadIdx.x; i0 < p.nrows; i0 += stride * HTB_U)
+	for (int64_t i = (int64_t) blockIdx.x * blockDim.x + threadIdx.x; i < p.nrows; i += stride)
 	{
-		uint32_t	h[HTB_U], pos[HTB_U], w[HTB_U], bits[HTB_U], word[HTB_U];
-		unsigned long long cur[HTB_U], e[HTB_U];
-		bool		v[HTB_U];
+		uint32_t	h = 0, w;
+		int64_t		key0 = 0;
+		bool		v = ht_row_hash(p.ht, (uint32_t) i, &h, &key0);
 
-#pragma unroll
-		for (int u = 0; u < HTB_U; u++)
+		if (v && !ht_in_batch(p.ht.nbatch, p.ht.batch_shift, p.ht.batch_id, h))
+			v = false;			/* another batch's row */
+		if (v && p.ht.keyslot && !ht_key_in_domain(p.ht.keyslot, key0))
 		{
-			const int64_t i = i0 + (int64_t) u * stride;
-			int64_t		key0 = 0;
-
-			h[u] = 0;
-			v[u] = i < p.nrows && ht_row_hash(p.ht, (uint32_t) i, &h[u], &key0);
-			if (v[u] && !ht_in_batch(p.ht.nbatch, p.ht.batch_shift, p.ht.batch_id, h[u]))
-				v[u] = false;		/* another batch's row */
-			if (v[u] && p.ht.keyslot && !ht_key_in_domain(p.ht.keyslot, key0))
-			{
-				outside = true;		/* the host builds the table again with hash values in the slots */
-				v[u] = false;
-			}
-			e[u] = ((unsigned long long) (p.ht.keyslot ? (uint32_t) key0 : h[u]) << 32) | (uint32_t) i;
-			pos[u] = h[u] & p.ht.mask;
-			bits[u] = ht_bloom_bits(h[u], &w[u], p.ht.bloom_mask);
+			outside = true;		/* the host builds the table again with hash values in the slots */
+			v = false;
 		}
+		const unsigned long long e = ((unsigned long long) (p.ht.keyslot ? (uint32_t) key0 : h) << 32) | (uint32_t) i;
+		uint32_t	pos = h & p.ht.mask;
+		const uint32_t bits = ht_bloom_bits(h, &w, p.ht.bloom_mask);
+
 		if (p.ht.bloom)
 		{
-#pragma unroll
-			for (int u = 0; u < HTB_U; u++)
-				word[u] = v[u] ? p.ht.bloom[w[u]] : 0xFFFFFFFFu;
-#pragma unroll
-			for (int u = 0; u < HTB_U; u++)
-				if ((word[u] & bits[u]) != bits[u])
-					atomicOr(p.ht.bloom + w[u], bits[u]);
-		}
-#pragma unroll
-		for (int u = 0; u < HTB_U; u++)
-			cur[u] = v[u] ? p.ht.slots[pos[u]] : 0;
-#pragma unroll
-		for (int u = 0; u < HTB_U; u++)
-		{
-			if (!v[u])
-				continue;
-			for (;;)
-			{
-				unsigned long long c = cur[u];
+			const uint32_t word = v ? p.ht.bloom[w] : 0xFFFFFFFFu;
 
-				if (c == HT_EMPTY)
-				{
-					c = atomicCAS(p.ht.slots + pos[u], HT_EMPTY, e[u]);
-					if (c == HT_EMPTY)
-						break;
-				}
-				/* occupied: the same key -> a duplicate on the build side (key-in-slot tables see it in the slot; the others
-				 * compare hash values first, then the keys by row id) */
-				if (!dup && (uint32_t) (c >> 32) == (uint32_t) (e[u] >> 32) &&
-					(p.ht.keyslot || ht_keys_equal_rows(p.ht, (uint32_t) c, (uint32_t) e[u])))
-					dup = true;
-				pos[u] = (pos[u] + 1) & p.ht.mask;
-				cur[u] = p.ht.slots[pos[u]];
-			}
-			inserted++;
+			if ((word & bits) != bits)
+				atomicOr(p.ht.bloom + w, bits);
 		}
+		if (!v)
+			continue;
+		unsigned long long cur = p.ht.slots[pos];
+
+		for (;;)
+		{
+			unsigned long long c = cur;
+
+			if (c == HT_EMPTY)
+			{
+				c = atomicCAS(p.ht.slots + pos, HT_EMPTY, e);
+				if (c == HT_EMPTY)
+					break;
+			}
+			/* occupied: the same key -> a duplicate on the build side (key-in-slot tables see it in the slot; the others
+			 * compare hash values first, then the keys by row id) */
+			if (!dup && (uint32_t) (c >> 32) == (uint32_t) (e >> 32) &&
+				(p.ht.keyslot || ht_keys_equal_rows(p.ht, (uint32_t) c, (uint32_t) e)))
+				dup = true;
+			pos = (pos + 1) & p.ht.mask;
+			cur = p.ht.slots[pos];
+		}
+		inserted++;
 	}
 	if (dup)
 		atomicExch(p.flags, 1);
@@ -174,17 +155,10 @@ ht_fill(cbgpu_hashtable *ht, int batch)
 		p.flags = ht->d_flags;
 		if (inner->nrows > 0)
 		{
-			const int	u = ctx->opt_htb_u;
-
-			blocks = (int) ((inner->nrows + 256 * u - 1) / (256 * u));
+			blocks = (int) ((inner->nrows + 255) / 256);
 			if (blocks > ctx->sm_count * 8)
 				blocks = ctx->sm_count * 8;
-			if (u == 4)
-				k_ht_build<4><<<blocks, 256, 0, ctx->stream>>>(p);
-			else if (u == 2)
-				k_ht_build<2><<<blocks, 256, 0, ctx->stream>>>(p);
-			else
-				k_ht_build<1><<<blocks, 256, 0, ctx->stream>>>(p);
+			k_ht_build<<<blocks, 256, 0, ctx->stream>>>(p);
 			CB_LAUNCHED(ctx, "k_ht_build");
 		}
 		CB_CUDA(ctx, cudaMemcpyAsync(h_flags, ht->d_flags, sizeof(h_flags), cudaMemcpyDeviceToHost, ctx->stream));
@@ -306,7 +280,7 @@ ht_create(cbgpu_ctx *ctx, cbgpu_rel *inner, const int32_t *keycols, int32_t nkey
 	CB_CUDA(ctx, cudaMallocAsync(&ht->d.slots, (size_t) nslots * sizeof(unsigned long long), ctx->stream));
 	CB_CUDA(ctx, cudaMallocAsync(&ht->d_flags, 3 * sizeof(int), ctx->stream));
 	/* one integer key: try the key-in-slot layout (int8 keys: as long as every build value lies in [0, 2^32)) */
-	if (nkeys == 1 && !ctx->opt_no_keyslot)
+	if (nkeys == 1)
 		switch (ht->d.keytype[0])
 		{
 			case CB_INT8:

@@ -35,12 +35,8 @@
 
 #define PC_THREADS 256
 #define PC_TILE 2048			/* driving rows per run of stage F                                    */
-#ifndef PC_BATCH
 #define PC_BATCH 1024			/* queue entries per run of any other stage                           */
-#endif
-#ifndef PC_OCC
 #define PC_OCC 4				/* resident CTAs per SM the register budget is set for                */
-#endif
 #define PC_U (PC_BATCH / PC_THREADS)
 #define PC_Q0CAP (PC_BATCH + PC_TILE)
 #define PC_QCAP (2 * PC_BATCH)	/* a consumer runs at PC_BATCH, a producer adds at most PC_BATCH      */
@@ -72,11 +68,11 @@ struct PcProbe
 	int32_t		kind;			/* 0: one int32 key, hashint4; 1: one int64 key, hashint8; 2: general */
 	PcCol		key[2];
 	int32_t		keytype[2];		/* hash function by the OUTER key's type (cross-type int4/int8 joins) */
-	/* how the table is reached.  0: Bloom filter stage B_j, then the table in HBM (stage H_j) - for build sides whose
-	 * tables miss L2.  1: ONE stage straight into the table - small build sides (L2-resident tables need no filter in
-	 * front of them).  2: the same, with the table's slots staged into the CTA's shared memory by a TMA bulk copy
-	 * (cp.async.bulk + mbarrier) when the kernel starts - dimension tables of a few thousand rows (nation, region, date):
-	 * such a probe never leaves the SM.  (nodeHash.c builds ONE table kind; SURVEY.md 8 row a6 asks for this split.) */
+	/* how the table is reached.  0: Bloom filter stage B_j, then the table in HBM (stage H_j).  1: ONE stage straight into
+	 * the table - the prefilter pass applied its Bloom filter already.  2: the same, with the table's slots staged into the
+	 * CTA's shared memory by a TMA bulk copy (cp.async.bulk + mbarrier) when the kernel starts - dimension tables of a few
+	 * thousand rows (nation, region, date): such a probe never leaves the SM.  (nodeHash.c builds ONE table kind;
+	 * SURVEY.md 8 row a6 asks for this split.) */
 	int32_t		mode;
 	int32_t		smem_off;		/* mode 2: first slot inside the dynamic shared memory, in slots       */
 };
@@ -115,7 +111,6 @@ struct PcParams
 	 * 16 bytes at a time like the qual columns) and feeds queue 1 directly: the rows the quals pass never
 	 * go through queue 0 and a separate gather of their keys */
 	int32_t		fuse0;
-	int32_t		spec0;			/* ... and its keys are loaded together with the qual columns after a dense tile */
 	uint32_t	smem_table_bytes;	/* shared-memory tables of the mode 2 probes, all together             */
 	/* sink */
 	int32_t		sink_kind;		/* CBP_SINK_AGG or CBP_SINK_MATERIALIZE                               */
@@ -888,8 +883,8 @@ struct PfParams
 	unsigned long long *out_count;
 };
 
-template <bool SPEC, int OCC>
-__global__ void __launch_bounds__(PC_THREADS, OCC)
+template <bool SPEC>
+__global__ void __launch_bounds__(PC_THREADS, SPEC ? 4 : 8)
 k_prefilter(const __grid_constant__ PfParams P)
 {
 	__shared__ uint32_t buf[PC_TILE];
@@ -913,7 +908,7 @@ k_prefilter(const __grid_constant__ PfParams P)
 		if (threadIdx.x == 0)
 			s_cnt = 0;
 		/* SPEC: the first filter's keys are requested together with the qual columns - one HBM latency per tile instead of
-		 * two, for 8 - 16 more registers per thread (4 resident CTAs instead of 6) */
+		 * two, for 8 - 16 more registers per thread (4 resident CTAs instead of 8) */
 		if (SPEC && P.nbloom > 0 && __all_sync(0xffffffffu, full))
 		{
 			keys0 = P.bloom[0].width == 8 ? pc_keys8_vec<true>(P.bloom[0].col, base + o0, pol_stream)
@@ -1012,216 +1007,6 @@ k_prefilter(const __grid_constant__ PfParams P)
 	}
 }
 
-/*
- * The same filter pass fed by a TMA ring (the shape of k_scan_agg_small): one persistent CTA per SM; a producer warp streams
- * every column the filters read - qual columns and filter key columns, a 1024-row tile at a time - into a ring of
- * shared-memory stages with bulk copies (cp.async.bulk + mbarrier), as many stages as fit ~168 KB, so HBM streams at
- * full rate whatever the consumers do.  Seven independent consumer groups of four warps take the tiles in turn (a tile's
- * critical path is one L2 round trip per Bloom filter: seven tiles in flight hide it); each thread owns 8 rows of its
- * group's tile, so 8 filter words are in flight per thread.  A group collects its survivors in shared memory (32-row runs
- * stay in row order) and appends them to the output with one global atomic per ~1000 survivors, not per tile.
- * The load-and-test version above (k_prefilter) needs one HBM latency per filter column and one L2 latency per filter,
- * one after the other, per tile, so it cannot keep HBM streaming at full rate.
- */
-#define PFT_TILE 1024
-#define PFT_GROUPS 7
-#define PFT_GTHREADS 128
-#define PFT_NCONS (PFT_GROUPS * PFT_GTHREADS)
-#define PFT_OBUF 1536			/* survivors a group holds back; flushed when a tile might not fit any more */
-#define PFT_MAXCOLS 8
-#define PFT_MAXSTAGES 28
-#define PFT_SMEM_BUDGET (168 * 1024)
-
-struct PftCol
-{
-	const void *data;
-	int32_t		width;			/* bytes per value: 1, 4 or 8                                         */
-	int32_t		off;			/* byte offset of the column inside a stage                           */
-};
-
-struct PftParams
-{
-	int64_t		nrows;
-	const uint8_t *visimap;
-	int32_t		ncols;
-	PftCol		col[PFT_MAXCOLS];
-	int32_t		nfilters;
-	int32_t		filt_col[2];	/* index into col[]                                                   */
-	int32_t		filt_lo[2];
-	uint32_t	filt_span[2];
-	int32_t		nbloom;
-	int32_t		bloom_col[PF_MAXBLOOM];
-	const uint32_t *bloom[PF_MAXBLOOM];
-	uint32_t	bloom_mask[PF_MAXBLOOM];
-	int32_t		nstages;
-	uint32_t	stage_bytes;
-	uint32_t   *out;
-	unsigned long long *out_count;
-};
-
-__global__ void __launch_bounds__(PFT_NCONS + 32, 1)
-k_prefilter_tma(const __grid_constant__ PftParams P)
-{
-	extern __shared__ __align__(128) unsigned char pft_smem[];
-	__shared__ uint64_t full_bar[PFT_MAXSTAGES];
-	__shared__ uint64_t empty_bar[PFT_MAXSTAGES];
-	__shared__ uint32_t obuf[PFT_GROUPS][PFT_OBUF];
-	__shared__ unsigned s_cnt[PFT_GROUPS];
-	__shared__ unsigned long long s_gbase[PFT_GROUPS];
-	const int	warp = threadIdx.x >> 5;
-	const int	lane = threadIdx.x & 31;
-	const int64_t ntiles = (P.nrows + PFT_TILE - 1) / PFT_TILE;
-	const int	nst = P.nstages;
-
-	if (threadIdx.x == 0)
-	{
-		for (int s = 0; s < nst; s++)
-		{
-			mbar_init(&full_bar[s], 1);
-			mbar_init(&empty_bar[s], PFT_GTHREADS / 32);
-		}
-		for (int g = 0; g < PFT_GROUPS; g++)
-			s_cnt[g] = 0;
-		asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-	}
-	__syncthreads();
-	if (warp == 0)
-	{
-		/* ---- producer ---- */
-		if (lane == 0)
-		{
-			int			it = 0;
-
-			for (int64_t t = blockIdx.x; t < ntiles; t += gridDim.x, it++)
-			{
-				const int	s = it % nst;
-				const unsigned ph = (unsigned) (it / nst) & 1;
-				const int64_t r0 = t * PFT_TILE;
-				const int64_t rows = P.nrows - r0 < PFT_TILE ? P.nrows - r0 : PFT_TILE;
-				unsigned char *st = pft_smem + (size_t) s * P.stage_bytes;
-				unsigned	total = 0;
-
-				/* bulk copies move multiples of 16 bytes; relations are allocated padded */
-				for (int c = 0; c < P.ncols; c++)
-					total += ((unsigned) (rows * P.col[c].width) + 15u) & ~15u;
-				mbar_wait(&empty_bar[s], ph ^ 1);
-				mbar_expect_tx(&full_bar[s], total);
-				for (int c = 0; c < P.ncols; c++)
-					tma_load_1d(st + P.col[c].off, (const unsigned char *) P.col[c].data + r0 * P.col[c].width,
-								((unsigned) (rows * P.col[c].width) + 15u) & ~15u, &full_bar[s]);
-			}
-		}
-		return;
-	}
-	/* ---- consumers: group g takes the CTA's tiles g, g + 7, g + 14, ... ---- */
-	{
-		const int	g = (threadIdx.x - 32) / PFT_GTHREADS;
-		const int	ct = (threadIdx.x - 32) % PFT_GTHREADS;
-		const uint64_t pol_keep = l2_policy_evict_last();
-		uint32_t   *const ob = obuf[g];
-		unsigned   *const cnt = &s_cnt[g];
-		const int	bar_id = 1 + g;
-		int			it = g;
-
-		for (int64_t t = blockIdx.x + (int64_t) g * gridDim.x; t < ntiles; t += (int64_t) PFT_GROUPS * gridDim.x, it += PFT_GROUPS)
-		{
-			const int	s = it % nst;
-			const unsigned ph = (unsigned) (it / nst) & 1;
-			const int64_t r0 = t * PFT_TILE;
-			const int	rows = (int) (P.nrows - r0 < PFT_TILE ? P.nrows - r0 : PFT_TILE);
-			const unsigned char *st = pft_smem + (size_t) s * P.stage_bytes;
-			unsigned	am = 0;
-
-			mbar_wait(&full_bar[s], ph);
-#pragma unroll
-			for (int j = 0; j < 8; j++)
-			{
-				const int	r = ct + j * PFT_GTHREADS;
-				bool		alive = r < rows;
-
-				if (alive && P.visimap)
-					alive = (__ldg(P.visimap + ((r0 + r) >> 3)) >> ((r0 + r) & 7)) & 1;
-				for (int f = 0; f < P.nfilters; f++)
-				{
-					const PftCol &c = P.col[P.filt_col[f]];
-					const int32_t v = c.width == 4 ? ((const int32_t *) (st + c.off))[r] : (int32_t) ((const uint8_t *) (st + c.off))[r];
-
-					alive = alive && (unsigned) (v - P.filt_lo[f]) <= P.filt_span[f];
-				}
-				am |= (unsigned) alive << j;
-			}
-			for (int f = 0; f < P.nbloom; f++)
-			{
-				const PftCol &c = P.col[P.bloom_col[f]];
-				uint32_t	bits[8], word[8];
-
-				if (!__any_sync(0xffffffffu, am != 0))
-					break;
-#pragma unroll
-				for (int j = 0; j < 8; j++)
-				{
-					const int	r = ct + j * PFT_GTHREADS;
-					uint32_t	w = 0;
-
-					bits[j] = 0;
-					word[j] = 0;
-					if ((am >> j) & 1)
-					{
-						const uint32_t h = c.width == 8 ? jh_int8(((const int64_t *) (st + c.off))[r])
-							: jh_mix32((uint32_t) ((const int32_t *) (st + c.off))[r]);
-
-						bits[j] = ht_bloom_bits(pg_hash_combine(0u, h, false), &w, P.bloom_mask[f]);
-						word[j] = ldg_hint_u32(P.bloom[f] + w, pol_keep);
-					}
-				}
-#pragma unroll
-				for (int j = 0; j < 8; j++)
-					if ((word[j] & bits[j]) != bits[j])
-						am &= ~(1u << j);
-			}
-			/* the stage's bytes are not needed any more: hand it back before the output work */
-			__syncwarp();
-			if (lane == 0)
-				mbar_arrive(&empty_bar[s]);
-			/* survivors -> the group's buffer: a warp's 32 consecutive rows of one j stay in order */
-#pragma unroll
-			for (int j = 0; j < 8; j++)
-			{
-				const unsigned m = __ballot_sync(0xffffffffu, (am >> j) & 1);
-				unsigned	wb = 0;
-
-				if (m == 0)
-					continue;
-				if (lane == 0)
-					wb = atomicAdd(cnt, (unsigned) __popc(m));
-				wb = __shfl_sync(0xffffffffu, wb, 0);
-				if ((am >> j) & 1)
-					ob[wb + __popc(m & ((1u << lane) - 1))] = (uint32_t) (r0 + ct + j * PFT_GTHREADS);
-			}
-			asm volatile("bar.sync %0, %1;" :: "r"(bar_id), "r"(PFT_GTHREADS) : "memory");	/* every push of this tile is in */
-			/* flush when the next tile might not fit, and after the group's last tile */
-			if (*cnt > PFT_OBUF - PFT_TILE || t + (int64_t) PFT_GROUPS * gridDim.x >= ntiles)
-			{
-				const unsigned n = *cnt;
-
-				if (ct == 0 && n)
-					s_gbase[g] = atomicAdd(P.out_count, (unsigned long long) n);
-				asm volatile("bar.sync %0, %1;" :: "r"(bar_id), "r"(PFT_GTHREADS) : "memory");
-				{
-					const unsigned long long gb = s_gbase[g];
-
-					for (unsigned i = ct; i < n; i += PFT_GTHREADS)
-						P.out[gb + i] = ob[i];
-				}
-				asm volatile("bar.sync %0, %1;" :: "r"(bar_id), "r"(PFT_GTHREADS) : "memory");	/* the buffer is free */
-				if (ct == 0)
-					*cnt = 0;
-				asm volatile("bar.sync %0, %1;" :: "r"(bar_id), "r"(PFT_GTHREADS) : "memory");
-			}
-		}
-	}
-}
-
 __global__ void __launch_bounds__(PC_THREADS, PC_OCC)
 k_probe_chain(const __grid_constant__ PcParams P)
 {
@@ -1242,7 +1027,6 @@ k_probe_chain(const __grid_constant__ PcParams P)
 	const int64_t ntiles = (P.nrows + tile_rows - 1) / tile_rows;
 	uint32_t   *const qg = P.qmem + (size_t) blockIdx.x * (size_t) P.q_cta_words;
 	int64_t		next_tile = blockIdx.x;	/* thread 0's */
-	bool		dense_prev = false;		/* this warp's previous tile: did most rows survive the quals?        */
 
 	if (threadIdx.x < PC_NQ)
 		cnt[threadIdx.x] = 0;
@@ -1328,17 +1112,7 @@ k_probe_chain(const __grid_constant__ PcParams P)
 			const bool	full = o0 + 8 <= nvalid;
 			const bool	wide0 = sprobe[0].kind == 1;
 			unsigned	am = 0;
-			PcKeys8		keys0;
-			bool		have_keys0 = false;
 
-			/* probe 0's keys ride along with the qual columns when this warp's previous tile was dense: their loads are
-			 * in flight together instead of one HBM latency after the other (late materialisation stays for sparse tiles) */
-			if (P.spec0 && dense_prev && __all_sync(0xffffffffu, full))
-			{
-				keys0 = wide0 ? pc_keys8_vec<true>(sprobe[0].key[0].data, base + o0, pol_stream)
-					: pc_keys8_vec<false>(sprobe[0].key[0].data, base + o0, pol_stream);
-				have_keys0 = true;
-			}
 			if (full)
 			{
 				int4		a0 = make_int4(0, 0, 0, 0), b0 = a0, a1 = a0, b1 = a0;
@@ -1394,23 +1168,14 @@ k_probe_chain(const __grid_constant__ PcParams P)
 			/* every lane votes (full-mask).  Only a warp whose rows mostly survived runs probe 0 here: its 8 hashes and
 			 * filter words per thread are work for live rows.  A sparse warp hands its few survivors to queue 0, where
 			 * stage B_0 will see them packed into full batches. */
-			const bool	dense = P.fuse0 && pc_warp_dense(full, am, 96u);
-
-			dense_prev = dense;
-			if (dense)
+			if (P.fuse0 && pc_warp_dense(full, am, 96u))
 			{
 				if (wide0)
-				{
-					if (!have_keys0)
-						keys0 = pc_keys8_vec<true>(sprobe[0].key[0].data, base + o0, pol_stream);
-					pc_stage_f_probe0<true>(sprobe[0], base + o0, keys0, am, qg + P.q_off[1], (unsigned) P.q_cap[1], &cnt[1]);
-				}
+					pc_stage_f_probe0<true>(sprobe[0], base + o0, pc_keys8_vec<true>(sprobe[0].key[0].data, base + o0, pol_stream), am,
+											qg + P.q_off[1], (unsigned) P.q_cap[1], &cnt[1]);
 				else
-				{
-					if (!have_keys0)
-						keys0 = pc_keys8_vec<false>(sprobe[0].key[0].data, base + o0, pol_stream);
-					pc_stage_f_probe0<false>(sprobe[0], base + o0, keys0, am, qg + P.q_off[1], (unsigned) P.q_cap[1], &cnt[1]);
-				}
+					pc_stage_f_probe0<false>(sprobe[0], base + o0, pc_keys8_vec<false>(sprobe[0].key[0].data, base + o0, pol_stream), am,
+											 qg + P.q_off[1], (unsigned) P.q_cap[1], &cnt[1]);
 				continue;
 			}
 			const unsigned c = __popc(am);
@@ -1858,7 +1623,7 @@ cb_try_probe_chain(cbgpu_ctx *ctx, const CbPipeline *p, const PipeDev *d, bool *
 	 * hash-table access instead of after several. */
 	void	   *early_mem[PC_MAXEARLY] = {NULL, NULL};
 
-	for (int k = 0; k < np && P.nearly < PC_MAXEARLY && !ctx->opt_no_early_filter; k++)
+	for (int k = 0; k < np && P.nearly < PC_MAXEARLY; k++)
 	{
 		PcEarlyBuild *Bp = (PcEarlyBuild *) cb_scratch(ctx, 4, sizeof(PcEarlyBuild));
 		if (!Bp)
@@ -1969,7 +1734,7 @@ cb_try_probe_chain(cbgpu_ctx *ctx, const CbPipeline *p, const PipeDev *d, bool *
 	bool		pf_bloom_done[PC_MAXP] = {false, false, false, false};	/* probe j's Bloom filter was applied by the prefilter pass */
 	bool		pf_cand[PC_MAXP] = {false, false, false, false};
 
-	if (!ctx->opt_no_prefilter && P.nrows >= ctx->opt_pf_min_rows && np >= 1)	/* below ~16 M rows the fused kernel's fixed costs win */
+	if (P.nrows >= ctx->opt_pf_min_rows && np >= 1)	/* below ~16 M rows the fused kernel's fixed costs win */
 	{
 		PfParams   *Fp = (PfParams *) cb_scratch(ctx, 6, sizeof(PfParams));
 
@@ -2009,96 +1774,22 @@ cb_try_probe_chain(cbgpu_ctx *ctx, const CbPipeline *p, const PipeDev *d, bool *
 		if (F.nbloom + F.nfilters > 0 && !known_unselective)
 		{
 			unsigned long long nsel = 0;
-			int			fb = ctx->sm_count * 6;
 			const int64_t ft = (P.nrows + PC_TILE - 1) / PC_TILE;
 
-			if (fb > ft)
-				fb = (int) ft;
 			CB_CUDA(ctx, cudaMallocAsync(&pf_sel, (size_t) P.nrows * sizeof(uint32_t), ctx->stream));
 			CB_CUDA(ctx, cudaMallocAsync(&pf_count, sizeof(unsigned long long), ctx->stream));
 			CB_CUDA(ctx, cudaMemsetAsync(pf_count, 0, sizeof(unsigned long long), ctx->stream));
 			F.out = pf_sel;
 			F.out_count = pf_count;
 			const int	pkl = cb_klog_begin(ctx, "k_prefilter");
-			{
-				/* the TMA-fed version when the filters' columns fit the ring (they do unless there are many wide ones) */
-				PftParams  *Tp = (PftParams *) cb_scratch(ctx, 7, sizeof(PftParams));
-				bool		tma = Tp != NULL && ctx->opt_prefilter_tma;
 
-				if (tma)
-				{
-					PftParams  &T = *Tp;
-					uint32_t	off = 0;
-
-					T.nrows = F.nrows;
-					T.visimap = F.visimap;
-					T.out = pf_sel;
-					T.out_count = pf_count;
-					auto colidx = [&](const void *data, int width) -> int
-					{
-						for (int c = 0; c < T.ncols; c++)
-							if (T.col[c].data == data)
-								return c;
-						if (T.ncols >= PFT_MAXCOLS || ((uintptr_t) data & 15) != 0)
-							return -1;
-						T.col[T.ncols].data = data;
-						T.col[T.ncols].width = width;
-						T.col[T.ncols].off = (int32_t) off;
-						off += ((uint32_t) PFT_TILE * (uint32_t) width + 127u) & ~127u;
-						return T.ncols++;
-					};
-					T.nfilters = F.nfilters;
-					for (int f = 0; f < F.nfilters && tma; f++)
-					{
-						T.filt_col[f] = colidx(F.filt[f].col, F.filt[f].width);
-						T.filt_lo[f] = F.filt[f].lo;
-						T.filt_span[f] = F.filt[f].span;
-						tma = T.filt_col[f] >= 0;
-					}
-					T.nbloom = F.nbloom;
-					for (int f = 0; f < F.nbloom && tma; f++)
-					{
-						T.bloom_col[f] = colidx(F.bloom[f].col, F.bloom[f].width);
-						T.bloom[f] = F.bloom[f].bloom;
-						T.bloom_mask[f] = F.bloom[f].mask;
-						tma = T.bloom_col[f] >= 0;
-					}
-					T.stage_bytes = off;
-					T.nstages = off ? (int32_t) (PFT_SMEM_BUDGET / off) : 0;
-					if (T.nstages > PFT_MAXSTAGES)
-						T.nstages = PFT_MAXSTAGES;
-					tma = tma && T.nstages >= 2;
-					if (tma)
-					{
-						static bool attr_done = false;
-						const int64_t tt = (T.nrows + PFT_TILE - 1) / PFT_TILE;
-						int			tb = ctx->sm_count;
-
-						if (!attr_done)
-						{
-							CB_CUDA(ctx, cudaFuncSetAttribute(k_prefilter_tma, cudaFuncAttributeMaxDynamicSharedMemorySize, PFT_SMEM_BUDGET));
-							attr_done = true;
-						}
-						if (tb > tt)
-							tb = (int) tt;
-						k_prefilter_tma<<<tb, PFT_NCONS + 32, (size_t) T.nstages * T.stage_bytes, ctx->stream>>>(T);
-						CB_LAUNCHED(ctx, "k_prefilter_tma");
-					}
-				}
-				if (!tma)
-				{
-					/* 32 registers per thread: all 64 warps of an SM resident.  (Tried: 6 CTAs at 40 registers - slower; the first
-					 * filter's keys requested together with the qual columns, 64 registers, 4 CTAs - slower still: this pass
-					 * lives on occupancy.) */
-					if (ctx->opt_pf_spec)
-						k_prefilter<true, 4><<<ctx->sm_count * 4 < ft ? ctx->sm_count * 4 : (int) ft, PC_THREADS, 0, ctx->stream>>>(F);
-					else if (ctx->opt_pf_occ6)
-						k_prefilter<false, 6><<<fb, PC_THREADS, 0, ctx->stream>>>(F);
-					else
-						k_prefilter<false, 8><<<ctx->sm_count * 8 < ft ? ctx->sm_count * 8 : (int) ft, PC_THREADS, 0, ctx->stream>>>(F);
-					CB_LAUNCHED(ctx, "k_prefilter");
-				}
-			}
+			/* 32 registers per thread: all 64 warps of an SM resident - this pass lives on occupancy.  CBGPU_PF_SPEC trades
+			 * that for the first filter's keys requested together with the qual columns (64 registers, 4 CTAs per SM). */
+			if (ctx->opt_pf_spec)
+				k_prefilter<true><<<ctx->sm_count * 4 < ft ? ctx->sm_count * 4 : (int) ft, PC_THREADS, 0, ctx->stream>>>(F);
+			else
+				k_prefilter<false><<<ctx->sm_count * 8 < ft ? ctx->sm_count * 8 : (int) ft, PC_THREADS, 0, ctx->stream>>>(F);
+			CB_LAUNCHED(ctx, "k_prefilter");
 			cb_klog_end(ctx, pkl);
 			CB_CUDA(ctx, cudaMemcpyAsync(&nsel, pf_count, sizeof(nsel), cudaMemcpyDeviceToHost, ctx->stream));
 			CB_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
@@ -2136,11 +1827,9 @@ cb_try_probe_chain(cbgpu_ctx *ctx, const CbPipeline *p, const PipeDev *d, bool *
 		blocks = (int) ntiles;
 	if (blocks < 1)
 		blocks = 1;				/* nothing survived the prefilter: one CTA finds no tile and leaves */
-	/* probe 0 rides in stage F when its one integer key is a column of the driving relation that can be read 16 bytes at
-	 * a time, and stage F exists at all (without quals / visimap / scan-level filters the tiles start at B_0 already) */
 	/* how each table is reached (PcProbe.mode): a few thousand slots -> staged into shared memory by TMA (32 KB per CTA for
-	 * all of them together: four CTAs per SM stay resident); everything else Bloom filter first, then the table (probing an
-	 * L2-resident table in place, mode 1, is kept behind CBGPU_L2_DIRECT=1: it measured slower) */
+	 * all of them together: four CTAs per SM stay resident); everything else Bloom filter first, then the table, unless the
+	 * prefilter pass applied that filter already */
 	{
 		uint32_t	smem_slots = 0;
 
@@ -2149,8 +1838,6 @@ cb_try_probe_chain(cbgpu_ctx *ctx, const CbPipeline *p, const PipeDev *d, bool *
 			const uint64_t bytes = ((uint64_t) P.probe[j].ht.mask + 1) * 8;
 
 			P.probe[j].mode = 0;
-			if (ctx->opt_no_smem_ht)
-				continue;
 			if (bytes <= 32768 && (smem_slots * 8 + bytes) <= 32768 && ((uintptr_t) P.probe[j].ht.slots & 15) == 0)
 			{
 				P.probe[j].mode = 2;
@@ -2159,15 +1846,13 @@ cb_try_probe_chain(cbgpu_ctx *ctx, const CbPipeline *p, const PipeDev *d, bool *
 			}
 			else if (pf_bloom_done[j])
 				P.probe[j].mode = 1;	/* the rows that reach it passed its Bloom filter in the prefilter pass: straight to the table */
-			else if (ctx->opt_l2_direct && bytes <= ((uint64_t) 16 << 20))
-				P.probe[j].mode = 1;	/* slower than the filter in front of the table: a selective build side's Bloom filter sits
-										 * in L1, its table does not - off unless asked for */
 		}
 		P.smem_table_bytes = smem_slots * 8;
 	}
+	/* probe 0 rides in stage F when its one integer key is a column of the driving relation that can be read 16 bytes at
+	 * a time, and stage F exists at all (without quals / visimap / scan-level filters the tiles start at B_0 already) */
 	P.fuse0 = !iota && np >= 1 && P.probe[0].mode == 0 && P.probe[0].nkeys == 1 && (P.probe[0].kind == 0 || P.probe[0].kind == 1) &&
-		P.probe[0].key[0].src == 0 && ((uintptr_t) P.probe[0].key[0].data & 15) == 0 && !ctx->opt_no_fuse0;
-	P.spec0 = P.fuse0 && !ctx->opt_no_spec0;
+		P.probe[0].key[0].src == 0 && ((uintptr_t) P.probe[0].key[0].data & 15) == 0;
 	for (int k = 1; k <= 2 * np; k++)
 	{
 		P.q_off[k] = (int32_t) words;
@@ -2177,7 +1862,7 @@ cb_try_probe_chain(cbgpu_ctx *ctx, const CbPipeline *p, const PipeDev *d, bool *
 	P.q_cta_words = words;
 	CB_CUDA(ctx, cudaMallocAsync(&P.qmem, (size_t) blocks * (size_t) (words ? words : 1) * sizeof(uint32_t), ctx->stream));
 	if (ctx->opt_debug)
-		fprintf(stderr, "k_probe_chain: modes %d %d %d %d (0 filter + HBM table, 1 table in L2, 2 table in shared memory: %u bytes) fuse0 %d\n",
+		fprintf(stderr, "k_probe_chain: modes %d %d %d %d (0 filter + HBM table, 1 table only, 2 table in shared memory: %u bytes) fuse0 %d\n",
 				P.probe[0].mode, P.probe[1].mode, P.probe[2].mode, P.probe[3].mode, P.smem_table_bytes, P.fuse0);
 	if (ctx->opt_debug)
 		fprintf(stderr, "k_probe_chain: np %d nrows %lld tiles %lld blocks %d queue words/CTA %lld filters %d sink %d kinds %d %d %d %d\n", np,
