@@ -359,7 +359,8 @@ k_scan_agg_small(const __grid_constant__ SmallAggParams P)
 	 * fails the audit).  |k - c| < 2^(max(bits c, bits k) + 1), likewise k2 + d; a product has at most
 	 * the sum of its factors' bit counts, a thread's partial sum at most bits(value) + bits(rows
 	 * accumulated); all must stay below 63 bits.  NARROW additionally needs every single-IMAD
-	 * operand (a, b, c, d, b*(k-c)) below 2^32. */
+	 * operand (a, b, c, d, b*(k-c)) in [0, 2^32): below 2^32 by the bit counts, and b*(k-c) not
+	 * negative, which holds when every c seen is at most k (c < 2^bc, so 2^bc - 1 <= k proves it). */
 	{
 		int			bab = 64 - __clzll(S.magAB),
 					bc = 64 - __clzll(S.magC),
@@ -380,6 +381,8 @@ k_scan_agg_small(const __grid_constant__ SmallAggParams P)
 		if (worst + brows >= 63)
 			atomicExch(P.audit, 1);
 		if (NARROW && (bab > 32 || bc > 32 || bd > 32 || ((MASK & 0x10) && brev > 32)))
+			atomicExch(P.audit, 1);
+		if (NARROW && (MASK & 0x10) && (P.k < 0 || bc > 62 || (long long) ((1ull << bc) - 1) > P.k))
 			atomicExch(P.audit, 1);
 		/* negative inputs: the unsigned narrow form and the bit-count bounds do not hold */
 		if ((long long) (S.magAB | S.magC | S.magD) < 0)
