@@ -34,6 +34,40 @@ class CbgpuPairs(C.Structure):
     _fields_ = [("npairs", C.c_int64), ("outer_idx", C.c_void_p), ("inner_idx", C.c_void_p)]
 
 
+class CbpOp(C.Structure):
+    """one op of a postfix program (include/cbgpu.h CbpOpCode)"""
+    _fields_ = [("code", C.c_int32), ("a", C.c_int32), ("imm", C.c_int64)]
+
+
+class CbpColumn(C.Structure):
+    """a column a program loads: device pointers, CbTypeId, and which row source addresses it"""
+    _fields_ = [("data", C.c_void_p), ("nulls", C.c_void_p), ("dict_hash", C.c_void_p), ("type", C.c_int32), ("src", C.c_int32)]
+
+
+class CbgpuJoinFilter(C.Structure):
+    """cbgpu_join_filter: the program cbgpu_ht_probe_pairs_filtered tests on every key-equal (outer, build) pair"""
+    _fields_ = [("ncols", C.c_int32), ("cols", C.POINTER(CbpColumn)), ("nops", C.c_int32), ("ops", C.POINTER(CbpOp))]
+
+
+# CbpOpCode
+(CBP_END, CBP_LOAD, CBP_CONST, CBP_ADD, CBP_SUB, CBP_MUL, CBP_FADD, CBP_FSUB, CBP_FMUL, CBP_I2F, CBP_EQ, CBP_NE, CBP_LT, CBP_LE,
+ CBP_GT, CBP_GE, CBP_FEQ, CBP_FNE, CBP_FLT, CBP_FLE, CBP_FGT, CBP_FGE, CBP_AND, CBP_OR, CBP_NOT, CBP_FILTER, CBP_PROBE, CBP_DUP,
+ CBP_POP, CBP_F8ORD) = range(30)
+
+
+def join_filter(cols, ops):
+    """cols: [(DeviceRelation, column index, src)]; ops: [(code, a, imm)].  The arrays ride on the returned struct."""
+    ca = (CbpColumn * max(len(cols), 1))()
+    for i, (rel, c, src) in enumerate(cols):
+        L = rel.ctx.L
+        ca[i] = CbpColumn(L.cbgpu_rel_col_devptr(rel.h, c), L.cbgpu_rel_nulls_dev(rel.h, c), L.cbgpu_rel_dict_hash_dev(rel.h, c),
+                          L.cbgpu_rel_col_type(rel.h, c), src)
+    oa = (CbpOp * max(len(ops), 1))(*[CbpOp(code, a, imm) for code, a, imm in ops])
+    f = CbgpuJoinFilter(len(cols), ca, len(ops), oa)
+    f._keep = (ca, oa)
+    return f
+
+
 class CbAggStateDatum(C.Structure):
     _fields_ = [("n", C.c_int64), ("lo", C.c_int64), ("hi", C.c_int64)]
 
@@ -333,6 +367,10 @@ def gpu():
             "cbgpu_ht_nbatch": (C.c_int, [vp]),
             "cbgpu_ht_load_batch": (C.c_int, [vp, i32]),
             "cbgpu_ht_probe_pairs_batched": (C.c_int, [vp, vp, vp, C.POINTER(i32), i32, i32, i32, vp, vp, vp, C.POINTER(i64)]),
+            "cbgpu_ht_probe_pairs_filtered": (C.c_int, [vp, vp, vp, C.POINTER(i32), i32, i32, C.POINTER(CbgpuJoinFilter), vp, vp, vp,
+                                                        C.POINTER(i64)]),
+            "cbgpu_rel_nulls_dev": (vp, [vp, i32]),
+            "cbgpu_rel_dict_hash_dev": (vp, [vp, i32]),
             "cbgpu_pairs_free": (None, [vp]),
             "cbgpu_merge_sorted_runs": (C.c_int, [vp, vp, C.POINTER(i32), C.POINTER(i32), C.POINTER(i32), i32, i32, C.POINTER(vp),
                                                   C.POINTER(i32)]),

@@ -1013,6 +1013,99 @@ hj_interrupted(void *arg)
 	return es->es_interrupt_pending && es->es_interrupt_pending(es);
 }
 
+/* codes are compared, so a filter comparing dictionary columns needs both coded by one dictionary (as the join keys do) */
+static int
+filter_dicts_shared(CbEState *es, CbStream *s, int e)
+{
+	const PExpr *x = &s->pe[e];
+
+	if (x->kind != PE_OP)
+		return CBGPU_OK;
+	if (x->op >= CBP_EQ && x->op <= CBP_GE && x->r >= 0 && s->pe[x->l].kind == PE_COL && s->pe[x->r].kind == PE_COL)
+	{
+		const CbpColumn *a = &s->pipe.cols[s->pe[x->l].col],
+				   *b = &s->pipe.cols[s->pe[x->r].col];
+
+		if ((a->type == CB_DICT8 || a->type == CB_DICT32) && a->dict_hash != b->dict_hash)
+			return es_fail(es, CBGPU_ERR_UNSUPPORTED, "join of dictionary columns coded by two different dictionaries (share one dictionary between the columns)");
+	}
+	TRY(filter_dicts_shared(es, s, x->l));
+	return x->r >= 0 ? filter_dicts_shared(es, s, x->r) : CBGPU_OK;
+}
+
+/* mark the OUTER_VAR (used[0]) and INNER_VAR (used[1]) attnos an expression reads; out-of-range ones are left for translate
+ * to refuse */
+static void
+filter_vars_used(const CbExpr *e, uint8_t used[2][MAX_OUT])
+{
+	if (e->tag == T_CbVar && (e->varno == CB_OUTER_VAR || e->varno == CB_INNER_VAR) && e->varattno >= 1 && e->varattno <= MAX_OUT)
+		used[e->varno == CB_INNER_VAR][e->varattno - 1] = 1;
+	if (e->tag == T_CbOpExpr || e->tag == T_CbBoolExpr)
+		for (int i = 0; i < e->nargs; i++)
+			filter_vars_used(e->args[i], used);
+}
+
+/* a hash join's joinqual as the program of a filtered pair probe (the AND of its members): OUTER_VARs read the materialised
+ * outer relation (source 0), INNER_VARs the build relation (source 1) */
+static int
+join_filter_program(CbEState *es, CbStream *fs, cbgpu_rel *orel, const PExpr *shape, int nouter, NodePriv *hp, const CbHashJoin *hj)
+{
+	int			fouter[MAX_OUT],
+				finner[MAX_OUT];
+	uint8_t		used[2][MAX_OUT];
+	int			e = -1,
+				c = 0;
+	VarCtx		vc;
+
+	/* only the columns the filter reads go into its column table (and to the device) */
+	memset(used, 0, sizeof(used));
+	for (int i = 0; i < hj->njoinquals; i++)
+		filter_vars_used(hj->joinqual[i], used);
+	for (int i = 0; i < nouter; i++)
+	{
+		fouter[i] = -1;
+		if (used[0][i])
+		{
+			if (shape[i].kind == PE_STATE)
+				return es_fail(es, CBGPU_ERR_UNSUPPORTED, "join filter over an aggregate transition state is not supported on the GPU path");
+			if ((fouter[i] = pe_col(fs, orel, c, 0, 0)) < 0)
+				return es_fail(es, CBGPU_ERR_UNSUPPORTED, "too many columns in one join filter");
+			fs->pe[fouter[i]].dscale = shape[i].dscale;
+		}
+		c += shape[i].kind == PE_STATE ? 3 : 1;
+	}
+	for (int i = 0; i < hp->inner_nout; i++)
+	{
+		finner[i] = -1;
+		if (used[1][i])
+		{
+			if (hp->inner_pe[i].kind == PE_STATE)
+				return es_fail(es, CBGPU_ERR_UNSUPPORTED, "join filter over an aggregate transition state is not supported on the GPU path");
+			if ((finner[i] = pe_col(fs, hp->inner_rel, hp->inner_map[i], 1, 0)) < 0)
+				return es_fail(es, CBGPU_ERR_UNSUPPORTED, "too many columns in one join filter");
+			fs->pe[finner[i]].dscale = hp->inner_pe[i].dscale;
+		}
+	}
+	memset(&vc, 0, sizeof(vc));
+	vc.es = es;
+	vc.s = fs;
+	vc.outer = fouter;
+	vc.nouter = nouter;
+	vc.inner = finner;
+	vc.ninner = hp->inner_nout;
+	for (int i = 0; i < hj->njoinquals; i++)
+	{
+		int			q;
+
+		TRY(translate(&vc, hj->joinqual[i], &q));
+		e = e < 0 ? q : pe_op(fs, CBP_AND, e, q, CB_BOOL, 0, 0);
+		if (e < 0)
+			return es_fail(es, CBGPU_ERR_UNSUPPORTED, "join filter too large for the GPU path");
+	}
+	TRY(filter_dicts_shared(es, fs, e));
+	return emit_expr(es, fs, e);
+}
+
 static int
 open_hashjoin(CbPlanState *ps, CbStream **out)
 {
@@ -1049,7 +1142,14 @@ open_hashjoin(CbPlanState *ps, CbStream **out)
 		if (s->pe[keys[k]].kind == PE_STATE)
 			return es_fail(es, CBGPU_ERR_UNSUPPORTED, "join key over a transition state");
 	}
-	if ((cbgpu_ht_has_duplicates(hp->ht) && (hj->jointype == CB_JOIN_INNER || hj->jointype == CB_JOIN_LEFT)) ||
+	/* a join filter (joinqual) decides which key-equal candidates match: INNER joins apply it to the joined rows, LEFT / SEMI /
+	 * ANTI joins inside the probe's walk (filtered), the others are not on this path */
+	const int	filtered = hj->njoinquals > 0 &&
+		(hj->jointype == CB_JOIN_LEFT || hj->jointype == CB_JOIN_SEMI || hj->jointype == CB_JOIN_ANTI);
+
+	if (hj->njoinquals > 0 && hj->jointype != CB_JOIN_INNER && !filtered)
+		return es_fail(es, CBGPU_ERR_UNSUPPORTED, "extra join quals on a non-inner hash join are not implemented on the GPU path");
+	if (filtered || (cbgpu_ht_has_duplicates(hp->ht) && (hj->jointype == CB_JOIN_INNER || hj->jointype == CB_JOIN_LEFT)) ||
 		hj->jointype == CB_JOIN_RIGHT || hj->jointype == CB_JOIN_FULL)
 	{
 		const int	fill_outer = hj->jointype == CB_JOIN_LEFT || hj->jointype == CB_JOIN_FULL;
@@ -1083,7 +1183,29 @@ open_hashjoin(CbPlanState *ps, CbStream **out)
 		if (me->owned.npairs >= 8)
 			return es_fail(es, CBGPU_ERR_UNSUPPORTED, "too many N:M joins under one node");
 		pairs = &me->owned.pairs[me->owned.npairs++];
-		if (cbgpu_ht_nbatch(hp->ht) > 1)
+		if (filtered)
+		{
+			/* the join filter over the materialised outer relation (source 0) and the build relation (source 1), handed to the
+			 * probe; both kinds of table, one batch or several, go through the one call */
+			CbStream   *fs = stream_new(me);
+			cbgpu_join_filter jf;
+			int64_t		passes = 0;
+			int			rc;
+
+			if (!fs)
+				return es_fail(es, CBGPU_ERR_NOMEM, "host memory for a join filter");
+			TRY(join_filter_program(es, fs, orel, shape, nouter, hp, hj));
+			jf.ncols = fs->pipe.ncols;
+			jf.cols = fs->pipe.cols;
+			jf.nops = fs->pipe.nops;
+			jf.ops = fs->pipe.ops;
+			rc = cbgpu_ht_probe_pairs_filtered(es->es_ctx, hp->ht, orel, keycols, hj->nhashkeys, hj->jointype, &jf, hj_interrupted, es,
+											   pairs, &passes);
+			es->es_hashjoin_batches_run += passes;
+			if (rc != CBGPU_OK)
+				return es_fail(es, rc, "%s", cbgpu_last_error(es->es_ctx));
+		}
+		else if (cbgpu_ht_nbatch(hp->ht) > 1)
 		{
 			/* a build side split into batches: one pass per batch, each probed by its own outer rows; the pairs of all passes
 			 * come back as one list, so nothing downstream knows */
@@ -1110,7 +1232,11 @@ open_hashjoin(CbPlanState *ps, CbStream **out)
 		s2->rows_in = s->rows_in;
 		nouter = s2->nout;
 		memcpy(outer, s2->out, sizeof(int) * (size_t) nouter);
-		TRY(inner_out_exprs(es, s2, hp, 1, fill_outer, inner));
+		if (hj->jointype == CB_JOIN_SEMI || hj->jointype == CB_JOIN_ANTI)
+			for (int i = 0; i < hp->inner_nout; i++)
+				inner[i] = -1;	/* no inner columns survive a semi / anti join */
+		else
+			TRY(inner_out_exprs(es, s2, hp, 1, fill_outer, inner));
 		s = s2;
 		vc.s = s;
 	}
@@ -1186,10 +1312,11 @@ open_hashjoin(CbPlanState *ps, CbStream **out)
 	vc.nouter = nouter;
 	vc.inner = inner;
 	vc.ninner = hp->inner_nout;
-	if ((hj->njoinquals > 0 || ps->plan->nquals > 0) && hj->jointype != CB_JOIN_INNER)
-		return es_fail(es, CBGPU_ERR_UNSUPPORTED, "extra join quals on a non-inner hash join are not implemented on the GPU path");
-	for (int i = 0; i < hj->njoinquals; i++)
-		TRY(emit_qual(&vc, hj->joinqual[i]));
+	if (!filtered)
+		for (int i = 0; i < hj->njoinquals; i++)
+			TRY(emit_qual(&vc, hj->joinqual[i]));
+	/* the plan's own qual (otherqual) filters the joined or NULL-extended row: a NULL inner value makes it NULL, which drops
+	 * the row (nodeHashjoin.c:590, 660) */
 	for (int i = 0; i < ps->plan->nquals; i++)
 		TRY(emit_qual(&vc, ps->plan->qual[i]));
 	{

@@ -14,6 +14,7 @@
  * then the key equality (hashqualclauses).
  */
 #include "common.cuh"
+#include "pipeline.cuh"
 
 #include <stdlib.h>
 
@@ -408,6 +409,17 @@ cbgpu_ht_key_dict_hash(const cbgpu_hashtable *ht, int32_t k)
  * count matches per outer row -> exclusive scan -> write pairs.  Output order is outer-row major,
  * so the pair list is deterministic.
  * --------------------------------------------------------------------------------------------- */
+/* the join filter of a filtered pair probe (cbgpu_ht_probe_pairs_filtered); ops == NULL: none */
+struct JoinFilterDev
+{
+	const CbpColumn *cols;		/* device copies of the program                                       */
+	const CbpOp *ops;
+	int32_t		nops;
+	int32_t		jointype;		/* CB_JOIN_LEFT, SEMI or ANTI                                         */
+	uint32_t   *decision;		/* SEMI / ANTI: [rows of the pass] the first passing build row, or 0xFFFFFFFF */
+	int		   *status;			/* the context's status word: CBGPU_ERR_OVERFLOW                      */
+};
+
 struct ProbeParams
 {
 	HtDev		ht;
@@ -424,6 +436,7 @@ struct ProbeParams
 	unsigned long long *counts;	/* [n + 1] match counts, then their exclusive scan                    */
 	uint32_t   *out_outer;
 	uint32_t   *out_inner;
+	JoinFilterDev f;
 };
 
 /* an outer row's key hash (ht_row_hash over the probe side's columns) and its batch: the bits ht_in_batch tests, and batch 0
@@ -447,6 +460,41 @@ ht_probe_row_batch(const ProbeParams &p, uint32_t row, int64_t *key, uint32_t *h
 	return (p.ht.nbatch <= 1 || isnull) ? 0 : (int32_t) (h >> p.ht.batch_shift);
 }
 
+/* an outer row's key, hash and batch (*mine: the resident batch is the row's own), and whether it needs the table at all: its
+ * key is not NULL, the Bloom filter may hold it, it lies in the key-in-slot domain and its batch is resident */
+__device__ __forceinline__ bool
+ht_probe_admits(const ProbeParams &p, uint32_t row, int64_t *key, uint32_t *h, bool *mine)
+{
+	bool		isnull;
+
+	*mine = ht_probe_row_batch(p, row, key, h, &isnull) == p.ht.batch_id || p.ht.nbatch <= 1;
+	if (!isnull && p.ht.bloom)
+	{
+		uint32_t	w;
+		uint32_t	bits = ht_bloom_bits(*h, &w, p.ht.bloom_mask);
+
+		if ((__ldg(p.ht.bloom + w) & bits) != bits)
+			isnull = true;		/* certainly absent */
+	}
+	if (!isnull && p.ht.keyslot && !ht_key_in_domain(p.ht.keyslot, key[0]))
+		isnull = true;			/* outside the build side's key domain: no partner */
+	if (!isnull && !*mine)
+		isnull = true;			/* multi-batch join: this row belongs to another pass */
+	return !isnull;
+}
+
+/* does slot entry e hold a build row whose key equals the outer row's (hash value first, then the key columns by row id)? */
+__device__ __forceinline__ bool
+ht_slot_key_equal(const ProbeParams &p, unsigned long long e, uint32_t h, const int64_t *key)
+{
+	if ((uint32_t) (e >> 32) != (p.ht.keyslot ? (uint32_t) key[0] : h))
+		return false;
+	for (int k = 0; k < p.ht.nkeys && !p.ht.keyslot; k++)
+		if (cb_load_widen(p.ht.keydata[k], p.ht.keytype[k], (uint32_t) e) != key[k])
+			return false;
+	return true;
+}
+
 template <bool WRITE>
 __global__ void __launch_bounds__(256)
 k_ht_probe_pairs(ProbeParams p)
@@ -459,24 +507,11 @@ k_ht_probe_pairs(ProbeParams p)
 		uint32_t	row = p.sel ? p.sel[i] : (uint32_t) i;
 		uint32_t	h;
 		int64_t		key[CBP_MAX_KEYS];
-		bool		isnull;
-		const bool	mine = ht_probe_row_batch(p, row, key, &h, &isnull) == p.ht.batch_id || p.ht.nbatch <= 1;
+		bool		mine;
 		unsigned long long cnt = 0;
 		unsigned long long base = WRITE ? p.counts[i] : 0;
 
-		if (!isnull && p.ht.bloom)
-		{
-			uint32_t	w;
-			uint32_t	bits = ht_bloom_bits(h, &w, p.ht.bloom_mask);
-
-			if ((__ldg(p.ht.bloom + w) & bits) != bits)
-				isnull = true;		/* certainly absent */
-		}
-		if (!isnull && p.ht.keyslot && !ht_key_in_domain(p.ht.keyslot, key[0]))
-			isnull = true;			/* outside the build side's key domain: no partner */
-		if (!isnull && !mine)
-			isnull = true;			/* multi-batch join: this row belongs to another pass */
-		if (!isnull)
+		if (ht_probe_admits(p, row, key, &h, &mine))
 		{
 			uint32_t	pos = h & p.ht.mask;
 
@@ -486,25 +521,16 @@ k_ht_probe_pairs(ProbeParams p)
 
 				if (e == HT_EMPTY)
 					break;
-				if ((uint32_t) (e >> 32) == (p.ht.keyslot ? (uint32_t) key[0] : h))
+				if (ht_slot_key_equal(p, e, h, key))
 				{
-					uint32_t	irow = (uint32_t) e;
-					bool		eq = true;
-
-					for (int k = 0; k < p.ht.nkeys && !p.ht.keyslot; k++)
-						if (cb_load_widen(p.ht.keydata[k], p.ht.keytype[k], irow) != key[k])
-							eq = false;
-					if (eq)
+					if (WRITE)
 					{
-						if (WRITE)
-						{
-							p.out_outer[base + cnt] = row;
-							p.out_inner[base + cnt] = irow;
-						}
-						else if (p.matched)
-							p.matched[irow] = 1;
-						cnt++;
+						p.out_outer[base + cnt] = row;
+						p.out_inner[base + cnt] = (uint32_t) e;
 					}
+					else if (p.matched)
+						p.matched[(uint32_t) e] = 1;
+					cnt++;
 				}
 				pos = (pos + 1) & p.ht.mask;
 			}
@@ -512,6 +538,117 @@ k_ht_probe_pairs(ProbeParams p)
 		if (p.left && cnt == 0 && mine)
 		{
 			/* no partner (or a NULL key, which never has one): the outer row survives with a NULL inner side */
+			if (WRITE)
+			{
+				p.out_outer[base] = row;
+				p.out_inner[base] = 0xFFFFFFFFu;
+			}
+			cnt = 1;
+		}
+		if (!WRITE)
+			p.counts[i] = cnt;
+	}
+}
+
+/* the join filter over one key-equal candidate (outer row orow, build row irow): true only for a non-NULL true result */
+__device__ __forceinline__ bool
+join_filter_passes(const JoinFilterDev &f, uint32_t orow, uint32_t irow)
+{
+	int64_t		st[CBP_STACK];
+	uint64_t	snull = 0;
+	int			sp = 0;
+
+	for (int pc = 0; pc < f.nops; pc++)
+	{
+		const CbpOp op = f.ops[pc];
+
+		if (op.code == CBP_LOAD)
+		{
+			const CbpColumn &c = f.cols[op.a];
+			const uint32_t r = c.src ? irow : orow;
+			const bool	isnull = c.nulls && c.nulls[r];
+
+			st[sp] = isnull ? 0 : cb_load_widen(c.data, c.type, r);
+			snull = isnull ? (snull | (1ull << sp)) : (snull & ~(1ull << sp));
+			sp++;
+		}
+		else
+			cbp_scalar_op(op, st, snull, sp, true, f.status);
+	}
+	return !(snull & 1) && st[0] != 0;
+}
+
+/* The pair probe of a LEFT / SEMI / ANTI join with a join filter: ExecScanHashBucket's walk (nodeHash.c:2255) with the joinqual
+ * tested on every key-equal candidate (nodeHashjoin.c:583-713).  SEMI / ANTI stop at the first passing candidate (single_match
+ * :626, :610) and walk once: the count pass keeps each row's decision, the write pass only emits it.  LEFT emits every passing
+ * pair, so its write pass walks again. */
+template <bool WRITE>
+__global__ void __launch_bounds__(256)
+k_ht_probe_filtered(ProbeParams p)
+{
+	int64_t		i = (int64_t) blockIdx.x * blockDim.x + threadIdx.x;
+	int64_t		stride = (int64_t) gridDim.x * blockDim.x;
+	const bool	left = p.f.jointype == CB_JOIN_LEFT;
+
+	for (; i < p.n; i += stride)
+	{
+		const uint32_t row = p.sel ? p.sel[i] : (uint32_t) i;
+
+		if (WRITE && !left)
+		{
+			const unsigned long long at = p.counts[i];
+
+			if (p.counts[i + 1] != at)
+			{
+				p.out_outer[at] = row;
+				p.out_inner[at] = p.f.decision[i];
+			}
+			continue;
+		}
+		uint32_t	h;
+		int64_t		key[CBP_MAX_KEYS];
+		bool		mine;
+		unsigned long long cnt = 0;
+		const unsigned long long base = WRITE ? p.counts[i] : 0;
+		uint32_t	first = 0xFFFFFFFFu;
+
+		if (ht_probe_admits(p, row, key, &h, &mine))
+		{
+			uint32_t	pos = h & p.ht.mask;
+
+			for (;;)
+			{
+				unsigned long long e = p.ht.slots[pos];
+
+				if (e == HT_EMPTY)
+					break;
+				if (ht_slot_key_equal(p, e, h, key) && join_filter_passes(p.f, row, (uint32_t) e))
+				{
+					if (!left)
+					{
+						first = (uint32_t) e;
+						break;
+					}
+					if (WRITE)
+					{
+						p.out_outer[base + cnt] = row;
+						p.out_inner[base + cnt] = (uint32_t) e;
+					}
+					cnt++;
+				}
+				pos = (pos + 1) & p.ht.mask;
+			}
+		}
+		if (!left)
+		{
+			/* SEMI: the row with its first passing partner; ANTI: the row when none passed (a NULL key included) */
+			p.f.decision[i] = first;
+			p.counts[i] = p.f.jointype == CB_JOIN_SEMI ? first != 0xFFFFFFFFu : (first == 0xFFFFFFFFu && mine);
+			continue;
+		}
+		if (cnt == 0 && mine)
+		{
+			/* no passing partner: the outer row survives once with a NULL inner side */
 			if (WRITE)
 			{
 				p.out_outer[base] = row;
@@ -698,29 +835,22 @@ k_ht_partition_write(int64_t n, int32_t nbatch, int64_t chunk, const uint16_t *r
 	}
 }
 
-static int	ht_probe_pairs(cbgpu_ctx *ctx, const cbgpu_hashtable *ht, cbgpu_rel *outer, const int32_t *keycols, int32_t nkeys,
-						   const uint32_t *sel, int64_t nsel, int left, int fill_inner, cbgpu_pairs *out);
-
-extern "C" int
-cbgpu_ht_probe_pairs_outer(cbgpu_ctx *ctx, const cbgpu_hashtable *ht, cbgpu_rel *outer, const int32_t *keycols, int32_t nkeys,
-						   int32_t fill_outer, int32_t fill_inner, cbgpu_pairs *out)
+/* the device and host buffers of a pair probe: freed by ht_probe whatever the outcome */
+struct BatchedProbe
 {
-	return ht_probe_pairs(ctx, ht, outer, keycols, nkeys, NULL, 0, fill_outer != 0, fill_inner != 0, out);
-}
-
-extern "C" int
-cbgpu_ht_probe_pairs(cbgpu_ctx *ctx, const cbgpu_hashtable *ht, cbgpu_rel *outer, const int32_t *keycols, int32_t nkeys,
-					 const uint32_t *sel, int64_t nsel, cbgpu_pairs *out)
-{
-	return ht_probe_pairs(ctx, ht, outer, keycols, nkeys, sel, nsel, 0, 0, out);
-}
-
-extern "C" int
-cbgpu_ht_probe_pairs_left(cbgpu_ctx *ctx, const cbgpu_hashtable *ht, cbgpu_rel *outer, const int32_t *keycols, int32_t nkeys,
-						  cbgpu_pairs *out)
-{
-	return ht_probe_pairs(ctx, ht, outer, keycols, nkeys, NULL, 0, 1, 0, out);
-}
+	uint16_t   *rowbatch;		/* [n] each outer row's batch                                              */
+	unsigned long long *hist;	/* [nbatch][partition CTAs] row counts, then their exclusive scan          */
+	unsigned long long *d_offsets;	/* [nbatch + 1] where each batch's run starts in rows                  */
+	unsigned long long *h_offsets;
+	uint32_t   *rows;			/* [n] outer row ids grouped by batch                                       */
+	unsigned long long *counts;	/* match counts of one run (or of the build rows), then their scan          */
+	uint8_t    *matched;		/* RIGHT / FULL: [inner rows], kept across all passes                       */
+	uint32_t   *decision;		/* SEMI / ANTI with a join filter: each row's decision in the current pass  */
+	CbpColumn  *fcols;			/* the join filter's columns and ops on the device                          */
+	CbpOp	   *fops;
+	uint32_t   *grow[2];		/* the output's next, larger arrays while they are being filled             */
+	int64_t		cap;			/* pairs the output arrays hold                                             */
+};
 
 /* the probe side's key columns of a pair probe */
 static int
@@ -744,34 +874,132 @@ probe_params(cbgpu_ctx *ctx, const cbgpu_hashtable *ht, cbgpu_rel *outer, const 
 	return CBGPU_OK;
 }
 
+/* a join filter checked op by op (the stack depth it reaches, what it leaves), then copied to the device */
 static int
-ht_probe_pairs(cbgpu_ctx *ctx, const cbgpu_hashtable *ht, cbgpu_rel *outer, const int32_t *keycols, int32_t nkeys,
-			   const uint32_t *sel, int64_t nsel, int left, int fill_inner, cbgpu_pairs *out)
+join_filter_to_dev(cbgpu_ctx *ctx, const cbgpu_join_filter *jf, int32_t jointype, BatchedProbe *b, JoinFilterDev *f)
 {
-	ProbeParams p;
-	int64_t		n = sel ? nsel : outer->nrows;
-	unsigned long long total = 0;
+	int			depth = 0;
+
+	if (jf->ncols < 0 || jf->ncols > CBP_MAX_COLS || (jf->ncols > 0 && !jf->cols))
+		return cb_fail(ctx, CBGPU_ERR_INVALID, "join filter with %s%lld columns (0 .. 40 expected)", "", jf->ncols);
+	if (jf->nops < 1 || jf->nops > CBP_MAX_OPS || !jf->ops)
+		return cb_fail(ctx, CBGPU_ERR_INVALID, "join filter with %s%lld ops (1 .. 128 expected)", "", jf->nops);
+	for (int k = 0; k < jf->ncols; k++)
+	{
+		const CbpColumn *c = &jf->cols[k];
+
+		if (c->src != 0 && c->src != 1)
+			return cb_fail(ctx, CBGPU_ERR_INVALID, "join filter column %s%lld: src is neither 0 (probe side) nor 1 (build side)", "", k);
+		if (c->type < CB_INT4 || c->type > CB_BOOL || !c->data)
+			return cb_fail(ctx, CBGPU_ERR_INVALID, "join filter column %s%lld: no data, or a type the filter cannot load", "", k);
+	}
+	for (int pc = 0; pc < jf->nops; pc++)
+	{
+		const CbpOp *op = &jf->ops[pc];
+		int			pops = 0;
+
+		switch (op->code)
+		{
+			case CBP_LOAD:
+				if (op->a < 0 || op->a >= jf->ncols)
+					return cb_fail(ctx, CBGPU_ERR_INVALID, "join filter op %s%lld loads a column it does not have", "", pc);
+				break;
+			case CBP_CONST:
+				break;
+			case CBP_DUP:
+				if (op->a < 0 || op->a >= depth)
+					return cb_fail(ctx, CBGPU_ERR_INVALID, "join filter op %s%lld copies a stack entry that is not there", "", pc);
+				break;
+			case CBP_POP:
+				pops = 1;
+				break;
+			case CBP_I2F: case CBP_F8ORD: case CBP_NOT:
+				pops = 1;
+				break;
+			case CBP_ADD: case CBP_SUB: case CBP_MUL: case CBP_FADD: case CBP_FSUB: case CBP_FMUL:
+			case CBP_EQ: case CBP_NE: case CBP_LT: case CBP_LE: case CBP_GT: case CBP_GE:
+			case CBP_FEQ: case CBP_FNE: case CBP_FLT: case CBP_FLE: case CBP_FGT: case CBP_FGE:
+			case CBP_AND: case CBP_OR:
+				pops = 2;
+				break;
+			default:
+				return cb_fail(ctx, CBGPU_ERR_INVALID, "join filter op %s%lld: opcode not supported in a join filter", "", pc);
+		}
+		if (depth < pops)
+			return cb_fail(ctx, CBGPU_ERR_INVALID, "join filter op %s%lld takes more values than the stack holds", "", pc);
+		depth += (op->code == CBP_POP ? 0 : 1) - pops;
+		if (depth > CBP_STACK)
+			return cb_fail(ctx, CBGPU_ERR_INVALID, "join filter stack deeper than %s%lld values", "", CBP_STACK);
+	}
+	if (depth != 1)
+		return cb_fail(ctx, CBGPU_ERR_INVALID, "join filter leaves %s%lld values (one expected)", "", depth);
+	CB_CUDA(ctx, cudaSetDevice(ctx->device));
+	if (jf->ncols > 0)
+	{
+		CB_CUDA(ctx, cudaMallocAsync(&b->fcols, sizeof(CbpColumn) * (size_t) jf->ncols, ctx->stream));
+		CB_CUDA(ctx, cudaMemcpyAsync(b->fcols, jf->cols, sizeof(CbpColumn) * (size_t) jf->ncols, cudaMemcpyHostToDevice, ctx->stream));
+	}
+	CB_CUDA(ctx, cudaMallocAsync(&b->fops, sizeof(CbpOp) * (size_t) jf->nops, ctx->stream));
+	CB_CUDA(ctx, cudaMemcpyAsync(b->fops, jf->ops, sizeof(CbpOp) * (size_t) jf->nops, cudaMemcpyHostToDevice, ctx->stream));
+	f->cols = b->fcols;
+	f->ops = b->fops;
+	f->nops = jf->nops;
+	f->jointype = jointype;
+	f->status = ctx->d_status;
+	return CBGPU_OK;
+}
+
+/* one count (write = false) or write pass over p.n probe rows: the filtered kernel when the probe has a join filter */
+static int
+probe_pass(cbgpu_ctx *ctx, const ProbeParams &p, int blocks, bool write)
+{
+	if (p.f.ops && write)
+	{
+		k_ht_probe_filtered<true><<<blocks, 256, 0, ctx->stream>>>(p);
+		CB_LAUNCHED(ctx, "k_ht_probe_filtered<write>");
+	}
+	else if (p.f.ops)
+	{
+		k_ht_probe_filtered<false><<<blocks, 256, 0, ctx->stream>>>(p);
+		CB_LAUNCHED(ctx, "k_ht_probe_filtered<count>");
+	}
+	else if (write)
+	{
+		k_ht_probe_pairs<true><<<blocks, 256, 0, ctx->stream>>>(p);
+		CB_LAUNCHED(ctx, "k_ht_probe_pairs<write>");
+	}
+	else
+	{
+		k_ht_probe_pairs<false><<<blocks, 256, 0, ctx->stream>>>(p);
+		CB_LAUNCHED(ctx, "k_ht_probe_pairs<count>");
+	}
+	return CBGPU_OK;
+}
+
+/* the probe of a one-batch table: count, one scan over the probe rows' (and for fill_inner the build rows') counts, write */
+static int
+ht_probe_single(cbgpu_ctx *ctx, const cbgpu_hashtable *ht, ProbeParams p, int fill_inner, BatchedProbe *b, cbgpu_pairs *out)
+{
+	const int64_t n = p.n;
 	const int64_t ninner = fill_inner ? ht->inner->nrows : 0;
+	unsigned long long total = 0;
 	int			rc;
 
-	memset(out, 0, sizeof(*out));
-	/* one pass sees the resident batch only: the probe rows of every other batch would be missing from the result */
-	if (ht->d.nbatch > 1)
-		return cb_fail(ctx, CBGPU_ERR_INVALID, "%sa table of %lld batches is probed for pairs by cbgpu_ht_probe_pairs_batched", "",
-					   ht->d.nbatch);
-	if ((rc = probe_params(ctx, ht, outer, keycols, nkeys, &p)) != CBGPU_OK)
-		return rc;
-	p.sel = sel;
-	p.n = n;
-	p.left = left;
 	p.ninner = ninner;
 	if (n + ninner == 0)
 		return CBGPU_OK;
-	CB_CUDA(ctx, cudaMallocAsync(&p.counts, (size_t) (n + ninner + 1) * sizeof(unsigned long long), ctx->stream));
+	CB_CUDA(ctx, cudaMallocAsync(&b->counts, (size_t) (n + ninner + 1) * sizeof(unsigned long long), ctx->stream));
+	p.counts = b->counts;
 	if (ninner)
 	{
-		CB_CUDA(ctx, cudaMallocAsync(&p.matched, (size_t) ninner, ctx->stream));
-		CB_CUDA(ctx, cudaMemsetAsync(p.matched, 0, (size_t) ninner, ctx->stream));
+		CB_CUDA(ctx, cudaMallocAsync(&b->matched, (size_t) ninner, ctx->stream));
+		CB_CUDA(ctx, cudaMemsetAsync(b->matched, 0, (size_t) ninner, ctx->stream));
+		p.matched = b->matched;
+	}
+	if (p.f.ops && p.f.jointype != CB_JOIN_LEFT && n)
+	{
+		CB_CUDA(ctx, cudaMallocAsync(&b->decision, (size_t) n * sizeof(uint32_t), ctx->stream));
+		p.f.decision = b->decision;
 	}
 	int			blocks = (int) ((n + 255) / 256);
 	int			iblocks = (int) ((ninner + 255) / 256);
@@ -780,11 +1008,8 @@ ht_probe_pairs(cbgpu_ctx *ctx, const cbgpu_hashtable *ht, cbgpu_rel *outer, cons
 		blocks = ctx->sm_count * 8;
 	if (iblocks > ctx->sm_count * 8)
 		iblocks = ctx->sm_count * 8;
-	if (n)
-	{
-		k_ht_probe_pairs<false><<<blocks, 256, 0, ctx->stream>>>(p);
-		CB_LAUNCHED(ctx, "k_ht_probe_pairs<count>");
-	}
+	if (n && (rc = probe_pass(ctx, p, blocks, false)) != CBGPU_OK)
+		return rc;
 	if (ninner)
 	{
 		k_ht_unmatched_count<<<iblocks, 256, 0, ctx->stream>>>(p);
@@ -795,12 +1020,7 @@ ht_probe_pairs(cbgpu_ctx *ctx, const cbgpu_hashtable *ht, cbgpu_rel *outer, cons
 	CB_CUDA(ctx, cudaMemcpyAsync(&total, p.counts + n + ninner, sizeof(total), cudaMemcpyDeviceToHost, ctx->stream));
 	CB_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
 	if (total > 0xFFFFFFF0ull)
-	{
-		cudaFreeAsync(p.counts, ctx->stream);
-		if (p.matched)
-			cudaFreeAsync(p.matched, ctx->stream);
 		return cb_fail(ctx, CBGPU_ERR_UNSUPPORTED, "join result of %s%lld pairs exceeds the GPU path's 32-bit row ids", "", (long long) total);
-	}
 	out->npairs = (int64_t) total;
 	if (total)
 	{
@@ -808,36 +1028,16 @@ ht_probe_pairs(cbgpu_ctx *ctx, const cbgpu_hashtable *ht, cbgpu_rel *outer, cons
 		CB_CUDA(ctx, cudaMalloc(&out->inner_idx, (size_t) total * sizeof(uint32_t)));
 		p.out_outer = out->outer_idx;
 		p.out_inner = out->inner_idx;
-		if (n)
-		{
-			k_ht_probe_pairs<true><<<blocks, 256, 0, ctx->stream>>>(p);
-			CB_LAUNCHED(ctx, "k_ht_probe_pairs<write>");
-		}
+		if (n && (rc = probe_pass(ctx, p, blocks, true)) != CBGPU_OK)
+			return rc;
 		if (ninner)
 		{
 			k_ht_unmatched_write<<<iblocks, 256, 0, ctx->stream>>>(p);
 			CB_LAUNCHED(ctx, "k_ht_unmatched_write");
 		}
 	}
-	if (p.matched)
-		CB_CUDA(ctx, cudaFreeAsync(p.matched, ctx->stream));
-	CB_CUDA(ctx, cudaFreeAsync(p.counts, ctx->stream));
 	return CBGPU_OK;
 }
-
-/* the device and host buffers of a batched pair probe: freed by cbgpu_ht_probe_pairs_batched whatever the outcome */
-struct BatchedProbe
-{
-	uint16_t   *rowbatch;		/* [n] each outer row's batch                                              */
-	unsigned long long *hist;	/* [nbatch][partition CTAs] row counts, then their exclusive scan          */
-	unsigned long long *d_offsets;	/* [nbatch + 1] where each batch's run starts in rows                  */
-	unsigned long long *h_offsets;
-	uint32_t   *rows;			/* [n] outer row ids grouped by batch                                       */
-	unsigned long long *counts;	/* match counts of one run (or of the build rows), then their scan          */
-	uint8_t    *matched;		/* RIGHT / FULL: [inner rows], kept across all passes                       */
-	uint32_t   *grow[2];		/* the output's next, larger arrays while they are being filled             */
-	int64_t		cap;			/* pairs the output arrays hold                                             */
-};
 
 /* room for `need` pairs in out, keeping the out->npairs written so far (capacity doubles: the copies stay linear) */
 static int
@@ -939,6 +1139,11 @@ ht_probe_batched(cbgpu_ctx *ctx, cbgpu_hashtable *ht, ProbeParams p, int fill_in
 	}
 	CB_CUDA(ctx, cudaMallocAsync(&b->counts, (size_t) ((maxrun > ninner ? maxrun : ninner) + 1) * sizeof(unsigned long long), ctx->stream));
 	p.counts = b->counts;
+	if (p.f.ops && p.f.jointype != CB_JOIN_LEFT && maxrun)
+	{
+		CB_CUDA(ctx, cudaMallocAsync(&b->decision, (size_t) maxrun * sizeof(uint32_t), ctx->stream));
+		p.f.decision = b->decision;
+	}
 	if (ninner)
 	{
 		CB_CUDA(ctx, cudaMallocAsync(&b->matched, (size_t) ninner, ctx->stream));
@@ -963,15 +1168,10 @@ ht_probe_batched(cbgpu_ctx *ctx, cbgpu_hashtable *ht, ProbeParams p, int fill_in
 		p.ht = ht->d;
 		p.sel = b->rows + b->h_offsets[batch];
 		p.n = m;
-		k_ht_probe_pairs<false><<<blocks, 256, 0, ctx->stream>>>(p);
-		CB_LAUNCHED(ctx, "k_ht_probe_pairs<count>");
-		if ((rc = pairs_append(ctx, b, &p, m, out, &any)) != CBGPU_OK)
+		if ((rc = probe_pass(ctx, p, blocks, false)) != CBGPU_OK || (rc = pairs_append(ctx, b, &p, m, out, &any)) != CBGPU_OK)
 			return rc;
-		if (any)
-		{
-			k_ht_probe_pairs<true><<<blocks, 256, 0, ctx->stream>>>(p);
-			CB_LAUNCHED(ctx, "k_ht_probe_pairs<write>");
-		}
+		if (any && (rc = probe_pass(ctx, p, blocks, true)) != CBGPU_OK)
+			return rc;
 	}
 	if (ninner)
 	{
@@ -996,31 +1196,39 @@ ht_probe_batched(cbgpu_ctx *ctx, cbgpu_hashtable *ht, ProbeParams p, int fill_in
 	return CBGPU_OK;
 }
 
-extern "C" int
-cbgpu_ht_probe_pairs_batched(cbgpu_ctx *ctx, cbgpu_hashtable *ht, cbgpu_rel *outer, const int32_t *keycols, int32_t nkeys,
-							 int32_t fill_outer, int32_t fill_inner, int (*interrupted)(void *arg), void *arg, cbgpu_pairs *out,
-							 int64_t *passes)
+/* every pair probe: the resident table alone (nbatch <= 1) or batch by batch, with a join filter when `filter` is set.  On
+ * failure *out is empty; the probe's own buffers are freed whatever the outcome. */
+static int
+ht_probe(cbgpu_ctx *ctx, cbgpu_hashtable *ht, cbgpu_rel *outer, const int32_t *keycols, int32_t nkeys, const uint32_t *sel,
+		 int64_t nsel, int left, int fill_inner, int32_t jointype, const cbgpu_join_filter *filter, int (*interrupted)(void *arg),
+		 void *arg, cbgpu_pairs *out, int64_t *passes)
 {
 	BatchedProbe b;
 	ProbeParams p;
 	int64_t		npasses = 0;
 	int			rc;
 
-	if (passes)
-		*passes = 0;
-	if (ht->d.nbatch <= 1)
-		return ht_probe_pairs(ctx, ht, outer, keycols, nkeys, NULL, 0, fill_outer != 0, fill_inner != 0, out);
 	memset(out, 0, sizeof(*out));
-	if ((rc = probe_params(ctx, ht, outer, keycols, nkeys, &p)) != CBGPU_OK)
-		return rc;
-	p.n = outer->nrows;
-	p.left = fill_outer != 0;
 	memset(&b, 0, sizeof(b));
-	rc = ht_probe_batched(ctx, ht, p, fill_inner != 0, interrupted, arg, &b, out, &npasses);
+	rc = probe_params(ctx, ht, outer, keycols, nkeys, &p);
+	if (rc == CBGPU_OK && filter)
+		rc = join_filter_to_dev(ctx, filter, jointype, &b, &p.f);
+	if (rc == CBGPU_OK)
+	{
+		p.sel = sel;
+		p.n = sel ? nsel : outer->nrows;
+		p.left = left;
+		if (ht->d.nbatch > 1)
+			rc = ht_probe_batched(ctx, ht, p, fill_inner, interrupted, arg, &b, out, &npasses);
+		else
+			rc = ht_probe_single(ctx, ht, p, fill_inner, &b, out);
+	}
+	if (rc == CBGPU_OK && filter)
+		rc = cb_check_status(ctx, "join filter");	/* integer overflow inside the filter */
 	if (passes)
 		*passes = npasses;
 	{
-		void	   *dev[] = {b.rowbatch, b.hist, b.d_offsets, b.rows, b.counts, b.matched};
+		void	   *dev[] = {b.rowbatch, b.hist, b.d_offsets, b.rows, b.counts, b.matched, b.decision, b.fcols, b.fops};
 
 		for (size_t k = 0; k < sizeof(dev) / sizeof(dev[0]); k++)
 			if (dev[k])
@@ -1033,6 +1241,65 @@ cbgpu_ht_probe_pairs_batched(cbgpu_ctx *ctx, cbgpu_hashtable *ht, cbgpu_rel *out
 	if (rc != CBGPU_OK)
 		cbgpu_pairs_free(out);
 	return rc;
+}
+
+/* the single-pass entry points: one pass sees the resident batch only, so the probe rows of every other batch would be missing */
+static int
+ht_probe_pairs(cbgpu_ctx *ctx, const cbgpu_hashtable *ht, cbgpu_rel *outer, const int32_t *keycols, int32_t nkeys,
+			   const uint32_t *sel, int64_t nsel, int left, int fill_inner, cbgpu_pairs *out)
+{
+	memset(out, 0, sizeof(*out));
+	if (ht->d.nbatch > 1)
+		return cb_fail(ctx, CBGPU_ERR_INVALID, "%sa table of %lld batches is probed for pairs by cbgpu_ht_probe_pairs_batched", "",
+					   ht->d.nbatch);
+	return ht_probe(ctx, (cbgpu_hashtable *) ht, outer, keycols, nkeys, sel, nsel, left, fill_inner, CB_JOIN_INNER, NULL, NULL,
+					NULL, out, NULL);
+}
+
+extern "C" int
+cbgpu_ht_probe_pairs_outer(cbgpu_ctx *ctx, const cbgpu_hashtable *ht, cbgpu_rel *outer, const int32_t *keycols, int32_t nkeys,
+						   int32_t fill_outer, int32_t fill_inner, cbgpu_pairs *out)
+{
+	return ht_probe_pairs(ctx, ht, outer, keycols, nkeys, NULL, 0, fill_outer != 0, fill_inner != 0, out);
+}
+
+extern "C" int
+cbgpu_ht_probe_pairs(cbgpu_ctx *ctx, const cbgpu_hashtable *ht, cbgpu_rel *outer, const int32_t *keycols, int32_t nkeys,
+					 const uint32_t *sel, int64_t nsel, cbgpu_pairs *out)
+{
+	return ht_probe_pairs(ctx, ht, outer, keycols, nkeys, sel, nsel, 0, 0, out);
+}
+
+extern "C" int
+cbgpu_ht_probe_pairs_left(cbgpu_ctx *ctx, const cbgpu_hashtable *ht, cbgpu_rel *outer, const int32_t *keycols, int32_t nkeys,
+						  cbgpu_pairs *out)
+{
+	return ht_probe_pairs(ctx, ht, outer, keycols, nkeys, NULL, 0, 1, 0, out);
+}
+
+extern "C" int
+cbgpu_ht_probe_pairs_batched(cbgpu_ctx *ctx, cbgpu_hashtable *ht, cbgpu_rel *outer, const int32_t *keycols, int32_t nkeys,
+							 int32_t fill_outer, int32_t fill_inner, int (*interrupted)(void *arg), void *arg, cbgpu_pairs *out,
+							 int64_t *passes)
+{
+	return ht_probe(ctx, ht, outer, keycols, nkeys, NULL, 0, fill_outer != 0, fill_inner != 0, CB_JOIN_INNER, NULL, interrupted,
+					arg, out, passes);
+}
+
+extern "C" int
+cbgpu_ht_probe_pairs_filtered(cbgpu_ctx *ctx, cbgpu_hashtable *ht, cbgpu_rel *outer, const int32_t *keycols, int32_t nkeys,
+							  int32_t jointype, const cbgpu_join_filter *filter, int (*interrupted)(void *arg), void *arg,
+							  cbgpu_pairs *out, int64_t *passes)
+{
+	memset(out, 0, sizeof(*out));
+	if (passes)
+		*passes = 0;
+	if (jointype != CB_JOIN_LEFT && jointype != CB_JOIN_SEMI && jointype != CB_JOIN_ANTI)
+		return cb_fail(ctx, CBGPU_ERR_INVALID, "cbgpu_ht_probe_pairs_filtered: join type %s%lld is not LEFT, SEMI or ANTI", "", jointype);
+	if (!filter)
+		return cb_fail(ctx, CBGPU_ERR_INVALID, "cbgpu_ht_probe_pairs_filtered: no join filter%s", "");
+	return ht_probe(ctx, ht, outer, keycols, nkeys, NULL, 0, jointype == CB_JOIN_LEFT, 0, jointype, filter, interrupted, arg, out,
+					passes);
 }
 
 extern "C" void

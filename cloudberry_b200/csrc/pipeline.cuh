@@ -148,6 +148,166 @@ sink_acc_update(const AggDev &t, int slot, int a, const CbpAcc &acc, const int64
 	}
 }
 
+__device__ __forceinline__ int
+fcmp_pg(double x, double y)
+{
+	/* float8_cmp_internal (include/utils/float.h): NaN equals NaN and sorts above everything */
+	if (x != x)
+		return (y != y) ? 0 : 1;
+	if (y != y)
+		return -1;
+	return x < y ? -1 : (x > y ? 1 : 0);
+}
+
+/* One scalar op of a postfix program over the value stack st[0 .. sp) with NULL bits snull: CONST, DUP, POP, integer and float8
+ * arithmetic, I2F, F8ORD, the compares and three-valued AND / OR / NOT.  The pipeline kernel and the join-filter probe both
+ * run their programs through it; each reads columns (LOAD) and consumes results (FILTER) itself.  Integer overflow of a live
+ * row (`alive`, operands not NULL) stores CBGPU_ERR_OVERFLOW in *status (int8pl / int8mi / int8mul report "bigint out of
+ * range", utils/adt/int8.c). */
+__device__ __forceinline__ void
+cbp_scalar_op(const CbpOp &op, int64_t *st, uint64_t &snull, int &sp, bool alive, int *status)
+{
+	const int	code = op.code;
+	const int	a = op.a;
+
+	switch (code)
+	{
+		case CBP_CONST:
+			st[sp] = op.imm;
+			snull &= ~(1ull << sp);
+			sp++;
+			break;
+		case CBP_DUP:
+			st[sp] = st[a];
+			snull = ((snull >> a) & 1) ? (snull | (1ull << sp)) : (snull & ~(1ull << sp));
+			sp++;
+			break;
+		case CBP_POP:
+			sp--;
+			break;
+		case CBP_ADD: case CBP_SUB: case CBP_MUL:
+			{
+				int64_t		y = st[sp - 1],
+							x = st[sp - 2];
+				bool		n = ((snull >> (sp - 1)) | (snull >> (sp - 2))) & 1;
+				int64_t		r;
+				bool		ovf;
+
+				/* scaled numerics share the check: a product that leaves 64 bits is refused, never wrapped */
+				if (code == CBP_ADD)
+				{
+					r = (int64_t) ((uint64_t) x + (uint64_t) y);
+					ovf = ((x ^ r) & (y ^ r)) < 0;
+				}
+				else if (code == CBP_SUB)
+				{
+					r = (int64_t) ((uint64_t) x - (uint64_t) y);
+					ovf = ((x ^ y) & (x ^ r)) < 0;
+				}
+				else
+				{
+					r = (int64_t) ((uint64_t) x * (uint64_t) y);
+					ovf = __mul64hi(x, y) != (r >> 63);
+				}
+				if (alive && !n && ovf)
+					atomicExch(status, CBGPU_ERR_OVERFLOW);
+				sp--;
+				st[sp - 1] = r;
+				snull = n ? (snull | (1ull << (sp - 1))) : (snull & ~(1ull << (sp - 1)));
+				break;
+			}
+		case CBP_FADD: case CBP_FSUB: case CBP_FMUL:
+			{
+				double		y = __longlong_as_double(st[sp - 1]),
+							x = __longlong_as_double(st[sp - 2]);
+				bool		n = ((snull >> (sp - 1)) | (snull >> (sp - 2))) & 1;
+				double		r = code == CBP_FADD ? __dadd_rn(x, y) : code == CBP_FSUB ? __dsub_rn(x, y) : __dmul_rn(x, y);
+
+				sp--;
+				st[sp - 1] = __double_as_longlong(r);
+				snull = n ? (snull | (1ull << (sp - 1))) : (snull & ~(1ull << (sp - 1)));
+				break;
+			}
+		case CBP_F8ORD:
+			{
+				long long	b = st[sp - 1];
+
+				if (__longlong_as_double(b) != __longlong_as_double(b))
+					b = 0x7FF8000000000000ll;	/* every NaN is the same value, above +Infinity */
+				st[sp - 1] = b >= 0 ? b : (b ^ 0x7FFFFFFFFFFFFFFFll);
+				break;
+			}
+		case CBP_I2F:
+			{
+				double		scale = 1.0;
+
+				for (int k = 0; k < a; k++)
+					scale *= 10.0;
+				st[sp - 1] = __double_as_longlong(__ddiv_rn((double) st[sp - 1], scale));
+				break;
+			}
+		case CBP_EQ: case CBP_NE: case CBP_LT: case CBP_LE: case CBP_GT: case CBP_GE:
+		case CBP_FEQ: case CBP_FNE: case CBP_FLT: case CBP_FLE: case CBP_FGT: case CBP_FGE:
+			{
+				int64_t		y = st[sp - 1],
+							x = st[sp - 2];
+				bool		n = ((snull >> (sp - 1)) | (snull >> (sp - 2))) & 1;
+				int			c;
+				bool		r;
+
+				if (code >= CBP_FEQ)
+					c = fcmp_pg(__longlong_as_double(x), __longlong_as_double(y));
+				else
+					c = x < y ? -1 : (x > y ? 1 : 0);
+				switch (code)
+				{
+					case CBP_EQ: case CBP_FEQ: r = c == 0; break;
+					case CBP_NE: case CBP_FNE: r = c != 0; break;
+					case CBP_LT: case CBP_FLT: r = c < 0; break;
+					case CBP_LE: case CBP_FLE: r = c <= 0; break;
+					case CBP_GT: case CBP_FGT: r = c > 0; break;
+					default: r = c >= 0; break;
+				}
+				sp--;
+				st[sp - 1] = r;
+				snull = n ? (snull | (1ull << (sp - 1))) : (snull & ~(1ull << (sp - 1)));
+				break;
+			}
+		case CBP_AND: case CBP_OR:
+			{
+				/* three-valued logic of ExecEvalBoolAnd/OrStep (execExprInterp.c) */
+				bool		yn = (snull >> (sp - 1)) & 1,
+							xn = (snull >> (sp - 2)) & 1;
+				bool		y = st[sp - 1] != 0,
+							x = st[sp - 2] != 0;
+				bool		r,
+							n;
+
+				if (code == CBP_AND)
+				{
+					bool		anyfalse = (!xn && !x) || (!yn && !y);
+
+					r = !anyfalse;
+					n = !anyfalse && (xn || yn);
+				}
+				else
+				{
+					bool		anytrue = (!xn && x) || (!yn && y);
+
+					r = anytrue;
+					n = !anytrue && (xn || yn);
+				}
+				sp--;
+				st[sp - 1] = r;
+				snull = n ? (snull | (1ull << (sp - 1))) : (snull & ~(1ull << (sp - 1)));
+				break;
+			}
+		case CBP_NOT:
+			st[sp - 1] = !st[sp - 1];
+			break;
+	}
+}
+
 __device__ __forceinline__ void
 sink_store(void *col, int type, uint64_t pos, int64_t v)
 {

@@ -336,6 +336,30 @@ int			cbgpu_ht_probe_pairs_outer(cbgpu_ctx *ctx, const cbgpu_hashtable *ht, cbgp
 int			cbgpu_ht_probe_pairs_batched(cbgpu_ctx *ctx, cbgpu_hashtable *ht, cbgpu_rel *outer, const int32_t *keycols,
 										 int32_t nkeys, int32_t fill_outer, int32_t fill_inner, int (*interrupted) (void *arg),
 										 void *arg, cbgpu_pairs *out, int64_t *passes);
+/* a join filter (the hash join's joinqual): a postfix program that must leave exactly one boolean.  Its columns address the
+ * probe relation's row (src 0) or the build relation's row (src 1) of a key-equal candidate pair.  Ops: LOAD, CONST, DUP,
+ * POP, integer and float8 arithmetic, I2F, F8ORD, the compares, AND / OR / NOT.  NULL or false: the pair does not match
+ * (ExecQual). */
+typedef struct cbgpu_join_filter
+{
+	int32_t		ncols;
+	const CbpColumn *cols;		/* host array; each column's pointers are device pointers             */
+	int32_t		nops;
+	const CbpOp *ops;			/* host array                                                         */
+} cbgpu_join_filter;
+/* the pair probe of a LEFT, SEMI or ANTI hash join with a join filter: each key-equal candidate (ExecScanHashBucket,
+ * nodeHash.c:2255) counts as a match only if `filter` passes for it (nodeHashjoin.c:583-713).  Pairs come in outer-row order
+ * within each batch:
+ *   SEMI: (row, first passing build row), at most one per row; NULL-keyed rows and rows with no passing candidate give none;
+ *   ANTI: (row, 0xFFFFFFFF) for every row with no passing candidate, NULL-keyed rows included;
+ *   LEFT: every passing pair, and (row, 0xFFFFFFFF) for a row with none.
+ * A one-batch table and a table split into batches are both taken; batches, `interrupted`, *passes and the clean-up on
+ * failure as in cbgpu_ht_probe_pairs_batched.  CBGPU_ERR_INVALID, before any launch, for another join type or a malformed
+ * filter (a column src other than 0 / 1, a column or op outside the supported set, a stack deeper than CBP_STACK, a program
+ * that does not leave exactly one value); CBGPU_ERR_OVERFLOW when the filter's integer arithmetic overflows on a pair. */
+int			cbgpu_ht_probe_pairs_filtered(cbgpu_ctx *ctx, cbgpu_hashtable *ht, cbgpu_rel *outer, const int32_t *keycols,
+										  int32_t nkeys, int32_t jointype, const cbgpu_join_filter *filter,
+										  int (*interrupted) (void *arg), void *arg, cbgpu_pairs *out, int64_t *passes);
 void		cbgpu_pairs_free(cbgpu_pairs *p);
 int			cbgpu_read_u32(cbgpu_ctx *ctx, const uint32_t *dev, int64_t n, uint32_t *host);
 /* small device scratch (sink row counters, index vectors): zero-filled allocation, read-back, free */
