@@ -45,7 +45,7 @@ class CbpColumn(C.Structure):
 
 
 class CbgpuJoinFilter(C.Structure):
-    """cbgpu_join_filter: the program cbgpu_ht_probe_pairs_filtered tests on every key-equal (outer, build) pair"""
+    """cbgpu_join_filter: the program cbgpu_ht_probe_pairs tests on every key-equal (outer, build) pair"""
     _fields_ = [("ncols", C.c_int32), ("cols", C.POINTER(CbpColumn)), ("nops", C.c_int32), ("ops", C.POINTER(CbpOp))]
 
 
@@ -357,18 +357,14 @@ def gpu():
             "cbgpu_rel_copy_rows": (C.c_int, [vp, i64, vp, i64, i64]),
             "cbgpu_rel_col_devptr": (vp, [vp, i32]),
             "cbgpu_rel_nbytes": (C.c_size_t, [vp]),
-            "cbgpu_ht_build": (C.c_int, [vp, vp, C.POINTER(i32), i32, C.POINTER(vp)]),
+            "cbgpu_ht_build": (C.c_int, [vp, vp, C.POINTER(i32), i32, i32, C.POINTER(vp)]),
             "cbgpu_ht_free": (None, [vp]),
             "cbgpu_ht_nrows": (i64, [vp]),
             "cbgpu_ht_has_duplicates": (C.c_int, [vp]),
-            "cbgpu_ht_probe_pairs": (C.c_int, [vp, vp, vp, C.POINTER(i32), i32, vp, i64, vp]),
-            "cbgpu_ht_probe_pairs_outer": (C.c_int, [vp, vp, vp, C.POINTER(i32), i32, i32, i32, vp]),
-            "cbgpu_ht_build_batched": (C.c_int, [vp, vp, C.POINTER(i32), i32, i32, C.POINTER(vp)]),
             "cbgpu_ht_nbatch": (C.c_int, [vp]),
             "cbgpu_ht_load_batch": (C.c_int, [vp, i32]),
-            "cbgpu_ht_probe_pairs_batched": (C.c_int, [vp, vp, vp, C.POINTER(i32), i32, i32, i32, vp, vp, vp, C.POINTER(i64)]),
-            "cbgpu_ht_probe_pairs_filtered": (C.c_int, [vp, vp, vp, C.POINTER(i32), i32, i32, C.POINTER(CbgpuJoinFilter), vp, vp, vp,
-                                                        C.POINTER(i64)]),
+            "cbgpu_ht_probe_pairs": (C.c_int, [vp, vp, vp, C.POINTER(i32), i32, i32, C.POINTER(CbgpuJoinFilter), vp, vp, vp,
+                                               C.POINTER(i64)]),
             "cbgpu_rel_nulls_dev": (vp, [vp, i32]),
             "cbgpu_rel_dict_hash_dev": (vp, [vp, i32]),
             "cbgpu_pairs_free": (None, [vp]),

@@ -965,10 +965,7 @@ hash_build(CbPlanState *hashps)
 
 		while (budget > 0 && nbatch < 4096 && cbgpu_ht_bytes_for((cbgpu_rel_nrows(rel) + nbatch - 1) / nbatch) > budget)
 			nbatch <<= 1;
-		if (nbatch > 1)
-			GPU(es, cbgpu_ht_build_batched(es->es_ctx, rel, keycols, h->nhashkeys, nbatch, &p->ht));
-		else
-			GPU(es, cbgpu_ht_build(es->es_ctx, rel, keycols, h->nhashkeys, &p->ht));
+		GPU(es, cbgpu_ht_build(es->es_ctx, rel, keycols, h->nhashkeys, nbatch, &p->ht));
 		hashps->instrument.hashjoin_nbatch = nbatch;
 	}
 	p->owned.hts[p->owned.nhts++] = p->ht;
@@ -1164,8 +1161,11 @@ open_hashjoin(CbPlanState *ps, CbStream **out)
 		int			nshape;
 		int32_t		keycols[CBP_MAX_KEYS];
 		cbgpu_pairs *pairs;
+		cbgpu_join_filter jf;
+		int64_t		passes = 0;
 		NodePriv   *me = np(ps);
-		int			c;
+		int			c,
+					rc;
 
 		/* append the key expressions as extra output columns so the probe can read them */
 		for (int k = 0; k < hj->nhashkeys; k++)
@@ -1185,12 +1185,8 @@ open_hashjoin(CbPlanState *ps, CbStream **out)
 		pairs = &me->owned.pairs[me->owned.npairs++];
 		if (filtered)
 		{
-			/* the join filter over the materialised outer relation (source 0) and the build relation (source 1), handed to the
-			 * probe; both kinds of table, one batch or several, go through the one call */
+			/* the join filter over the materialised outer relation (source 0) and the build relation (source 1) */
 			CbStream   *fs = stream_new(me);
-			cbgpu_join_filter jf;
-			int64_t		passes = 0;
-			int			rc;
 
 			if (!fs)
 				return es_fail(es, CBGPU_ERR_NOMEM, "host memory for a join filter");
@@ -1199,26 +1195,14 @@ open_hashjoin(CbPlanState *ps, CbStream **out)
 			jf.cols = fs->pipe.cols;
 			jf.nops = fs->pipe.nops;
 			jf.ops = fs->pipe.ops;
-			rc = cbgpu_ht_probe_pairs_filtered(es->es_ctx, hp->ht, orel, keycols, hj->nhashkeys, hj->jointype, &jf, hj_interrupted, es,
-											   pairs, &passes);
-			es->es_hashjoin_batches_run += passes;
-			if (rc != CBGPU_OK)
-				return es_fail(es, rc, "%s", cbgpu_last_error(es->es_ctx));
 		}
-		else if (cbgpu_ht_nbatch(hp->ht) > 1)
-		{
-			/* a build side split into batches: one pass per batch, each probed by its own outer rows; the pairs of all passes
-			 * come back as one list, so nothing downstream knows */
-			int64_t		passes = 0;
-			int			rc = cbgpu_ht_probe_pairs_batched(es->es_ctx, hp->ht, orel, keycols, hj->nhashkeys, fill_outer, fill_inner,
-														  hj_interrupted, es, pairs, &passes);
-
-			es->es_hashjoin_batches_run += passes;
-			if (rc != CBGPU_OK)
-				return es_fail(es, rc, "%s", cbgpu_last_error(es->es_ctx));
-		}
-		else
-			GPU(es, cbgpu_ht_probe_pairs_outer(es->es_ctx, hp->ht, orel, keycols, hj->nhashkeys, fill_outer, fill_inner, pairs));
+		/* a build side split into batches gets one pass per batch, each probed by its own outer rows; the pairs of all passes
+		 * come back as one list, so nothing downstream knows */
+		rc = cbgpu_ht_probe_pairs(es->es_ctx, hp->ht, orel, keycols, hj->nhashkeys, hj->jointype, filtered ? &jf : NULL,
+								  hj_interrupted, es, pairs, &passes);
+		es->es_hashjoin_batches_run += passes;
+		if (rc != CBGPU_OK)
+			return es_fail(es, rc, "%s", cbgpu_last_error(es->es_ctx));
 		s2 = stream_new(me);
 		TRY(stream_over_rel(es, s2, orel, shape, nouter));
 		if (fill_inner)

@@ -308,21 +308,6 @@ ht_create(cbgpu_ctx *ctx, cbgpu_rel *inner, const int32_t *keycols, int32_t nkey
 	return CBGPU_OK;
 }
 
-extern "C" int
-cbgpu_ht_build(cbgpu_ctx *ctx, cbgpu_rel *inner, const int32_t *keycols, int32_t nkeys, cbgpu_hashtable **out)
-{
-	int			rc = ht_create(ctx, inner, keycols, nkeys, 1, out);
-
-	if (rc == CBGPU_OK)
-		rc = ht_fill(*out, 0);
-	if (rc != CBGPU_OK && *out)
-	{
-		cbgpu_ht_free(*out);
-		*out = NULL;
-	}
-	return rc;
-}
-
 /* what a single-batch table over `rows` build rows takes on the device (slots at load factor <= 0.5 + the filter):
  * the caller's figure for choosing nbatch against its memory budget (ExecChooseHashTableSize, nodeHash.c:856-1100) */
 extern "C" int64_t
@@ -339,7 +324,7 @@ cbgpu_ht_bytes_for(int64_t rows)
 }
 
 extern "C" int
-cbgpu_ht_build_batched(cbgpu_ctx *ctx, cbgpu_rel *inner, const int32_t *keycols, int32_t nkeys, int32_t nbatch, cbgpu_hashtable **out)
+cbgpu_ht_build(cbgpu_ctx *ctx, cbgpu_rel *inner, const int32_t *keycols, int32_t nkeys, int32_t nbatch, cbgpu_hashtable **out)
 {
 	int			rc = ht_create(ctx, inner, keycols, nkeys, nbatch, out);
 
@@ -409,7 +394,7 @@ cbgpu_ht_key_dict_hash(const cbgpu_hashtable *ht, int32_t k)
  * count matches per outer row -> exclusive scan -> write pairs.  Output order is outer-row major,
  * so the pair list is deterministic.
  * --------------------------------------------------------------------------------------------- */
-/* the join filter of a filtered pair probe (cbgpu_ht_probe_pairs_filtered); ops == NULL: none */
+/* the join filter of a filtered pair probe; ops == NULL: none */
 struct JoinFilterDev
 {
 	const CbpColumn *cols;		/* device copies of the program                                       */
@@ -835,15 +820,15 @@ k_ht_partition_write(int64_t n, int32_t nbatch, int64_t chunk, const uint16_t *r
 	}
 }
 
-/* the device and host buffers of a pair probe: freed by ht_probe whatever the outcome */
-struct BatchedProbe
+/* the device and host buffers of a pair probe: freed by cbgpu_ht_probe_pairs whatever the outcome */
+struct PairProbe
 {
 	uint16_t   *rowbatch;		/* [n] each outer row's batch                                              */
 	unsigned long long *hist;	/* [nbatch][partition CTAs] row counts, then their exclusive scan          */
 	unsigned long long *d_offsets;	/* [nbatch + 1] where each batch's run starts in rows                  */
 	unsigned long long *h_offsets;
 	uint32_t   *rows;			/* [n] outer row ids grouped by batch                                       */
-	unsigned long long *counts;	/* match counts of one run (or of the build rows), then their scan          */
+	unsigned long long *counts;	/* match counts of one run (the last also of the build rows), then their scan */
 	uint8_t    *matched;		/* RIGHT / FULL: [inner rows], kept across all passes                       */
 	uint32_t   *decision;		/* SEMI / ANTI with a join filter: each row's decision in the current pass  */
 	CbpColumn  *fcols;			/* the join filter's columns and ops on the device                          */
@@ -876,7 +861,7 @@ probe_params(cbgpu_ctx *ctx, const cbgpu_hashtable *ht, cbgpu_rel *outer, const 
 
 /* a join filter checked op by op (the stack depth it reaches, what it leaves), then copied to the device */
 static int
-join_filter_to_dev(cbgpu_ctx *ctx, const cbgpu_join_filter *jf, int32_t jointype, BatchedProbe *b, JoinFilterDev *f)
+join_filter_to_dev(cbgpu_ctx *ctx, const cbgpu_join_filter *jf, int32_t jointype, PairProbe *b, JoinFilterDev *f)
 {
 	int			depth = 0;
 
@@ -976,72 +961,9 @@ probe_pass(cbgpu_ctx *ctx, const ProbeParams &p, int blocks, bool write)
 	return CBGPU_OK;
 }
 
-/* the probe of a one-batch table: count, one scan over the probe rows' (and for fill_inner the build rows') counts, write */
-static int
-ht_probe_single(cbgpu_ctx *ctx, const cbgpu_hashtable *ht, ProbeParams p, int fill_inner, BatchedProbe *b, cbgpu_pairs *out)
-{
-	const int64_t n = p.n;
-	const int64_t ninner = fill_inner ? ht->inner->nrows : 0;
-	unsigned long long total = 0;
-	int			rc;
-
-	p.ninner = ninner;
-	if (n + ninner == 0)
-		return CBGPU_OK;
-	CB_CUDA(ctx, cudaMallocAsync(&b->counts, (size_t) (n + ninner + 1) * sizeof(unsigned long long), ctx->stream));
-	p.counts = b->counts;
-	if (ninner)
-	{
-		CB_CUDA(ctx, cudaMallocAsync(&b->matched, (size_t) ninner, ctx->stream));
-		CB_CUDA(ctx, cudaMemsetAsync(b->matched, 0, (size_t) ninner, ctx->stream));
-		p.matched = b->matched;
-	}
-	if (p.f.ops && p.f.jointype != CB_JOIN_LEFT && n)
-	{
-		CB_CUDA(ctx, cudaMallocAsync(&b->decision, (size_t) n * sizeof(uint32_t), ctx->stream));
-		p.f.decision = b->decision;
-	}
-	int			blocks = (int) ((n + 255) / 256);
-	int			iblocks = (int) ((ninner + 255) / 256);
-
-	if (blocks > ctx->sm_count * 8)
-		blocks = ctx->sm_count * 8;
-	if (iblocks > ctx->sm_count * 8)
-		iblocks = ctx->sm_count * 8;
-	if (n && (rc = probe_pass(ctx, p, blocks, false)) != CBGPU_OK)
-		return rc;
-	if (ninner)
-	{
-		k_ht_unmatched_count<<<iblocks, 256, 0, ctx->stream>>>(p);
-		CB_LAUNCHED(ctx, "k_ht_unmatched_count");
-	}
-	k_exclusive_scan_u64<<<1, 1024, 0, ctx->stream>>>(p.counts, n + ninner);
-	CB_LAUNCHED(ctx, "k_exclusive_scan_u64");
-	CB_CUDA(ctx, cudaMemcpyAsync(&total, p.counts + n + ninner, sizeof(total), cudaMemcpyDeviceToHost, ctx->stream));
-	CB_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-	if (total > 0xFFFFFFF0ull)
-		return cb_fail(ctx, CBGPU_ERR_UNSUPPORTED, "join result of %s%lld pairs exceeds the GPU path's 32-bit row ids", "", (long long) total);
-	out->npairs = (int64_t) total;
-	if (total)
-	{
-		CB_CUDA(ctx, cudaMalloc(&out->outer_idx, (size_t) total * sizeof(uint32_t)));
-		CB_CUDA(ctx, cudaMalloc(&out->inner_idx, (size_t) total * sizeof(uint32_t)));
-		p.out_outer = out->outer_idx;
-		p.out_inner = out->inner_idx;
-		if (n && (rc = probe_pass(ctx, p, blocks, true)) != CBGPU_OK)
-			return rc;
-		if (ninner)
-		{
-			k_ht_unmatched_write<<<iblocks, 256, 0, ctx->stream>>>(p);
-			CB_LAUNCHED(ctx, "k_ht_unmatched_write");
-		}
-	}
-	return CBGPU_OK;
-}
-
 /* room for `need` pairs in out, keeping the out->npairs written so far (capacity doubles: the copies stay linear) */
 static int
-pairs_reserve(cbgpu_ctx *ctx, BatchedProbe *b, cbgpu_pairs *out, int64_t need)
+pairs_reserve(cbgpu_ctx *ctx, PairProbe *b, cbgpu_pairs *out, int64_t need)
 {
 	const int64_t cap = b->cap * 2 > need ? b->cap * 2 : need;
 
@@ -1068,7 +990,7 @@ pairs_reserve(cbgpu_ctx *ctx, BatchedProbe *b, cbgpu_pairs *out, int64_t need)
 
 /* the pairs whose counts p.counts[0 .. nc) holds, appended to out: scan, one read-back, room, then `write` */
 static int
-pairs_append(cbgpu_ctx *ctx, BatchedProbe *b, ProbeParams *p, int64_t nc, cbgpu_pairs *out, bool *any)
+pairs_append(cbgpu_ctx *ctx, PairProbe *b, ProbeParams *p, int64_t nc, cbgpu_pairs *out, bool *any)
 {
 	unsigned long long t = 0;
 
@@ -1092,14 +1014,19 @@ pairs_append(cbgpu_ctx *ctx, BatchedProbe *b, ProbeParams *p, int64_t nc, cbgpu_
 	return CBGPU_OK;
 }
 
+/* HJ_NEED_NEW_BATCH (nodeHashjoin.c:709-738): each batch resident in turn, probed by its own run of outer rows.  A one-batch
+ * table is one run of every outer row in relation order over the table as built: nothing is partitioned or reloaded.  The
+ * last run also counts the build rows left unmatched (every count pass has marked its matches by then), so one scan and one
+ * read-back serve both. */
 static int
-ht_probe_batched(cbgpu_ctx *ctx, cbgpu_hashtable *ht, ProbeParams p, int fill_inner, int (*interrupted)(void *arg), void *arg,
-				 BatchedProbe *b, cbgpu_pairs *out, int64_t *passes)
+ht_probe_batches(cbgpu_ctx *ctx, cbgpu_hashtable *ht, ProbeParams p, int fill_inner, int (*interrupted)(void *arg), void *arg,
+				 PairProbe *b, cbgpu_pairs *out, int64_t *passes)
 {
 	const int32_t nbatch = ht->d.nbatch;
 	const int64_t n = p.n;
 	const int64_t ninner = fill_inner ? ht->inner->nrows : 0;
 	int64_t		maxrun = 0;
+	int			iblocks = (int) ((ninner + 255) / 256);
 	bool		any;
 	int			rc;
 
@@ -1107,7 +1034,9 @@ ht_probe_batched(cbgpu_ctx *ctx, cbgpu_hashtable *ht, ProbeParams p, int fill_in
 	b->h_offsets = (unsigned long long *) calloc((size_t) nbatch + 1, sizeof(unsigned long long));
 	if (!b->h_offsets)
 		return cb_fail(ctx, CBGPU_ERR_NOMEM, "host memory for %s%lld batch offsets", "", nbatch);
-	if (n > 0)
+	if (nbatch == 1)
+		b->h_offsets[1] = (unsigned long long) n;
+	else if (n > 0)
 	{
 		/* at most 2^18 [batch][CTA] counts: the scan over them runs on one CTA */
 		int64_t		grid = (int64_t) ctx->sm_count * 2,
@@ -1133,11 +1062,11 @@ ht_probe_batched(cbgpu_ctx *ctx, cbgpu_hashtable *ht, ProbeParams p, int fill_in
 		CB_CUDA(ctx, cudaMemcpyAsync(b->h_offsets, b->d_offsets, ((size_t) nbatch + 1) * sizeof(unsigned long long),
 									 cudaMemcpyDeviceToHost, ctx->stream));
 		CB_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-		for (int32_t k = 0; k < nbatch; k++)
-			if ((int64_t) (b->h_offsets[k + 1] - b->h_offsets[k]) > maxrun)
-				maxrun = (int64_t) (b->h_offsets[k + 1] - b->h_offsets[k]);
 	}
-	CB_CUDA(ctx, cudaMallocAsync(&b->counts, (size_t) ((maxrun > ninner ? maxrun : ninner) + 1) * sizeof(unsigned long long), ctx->stream));
+	for (int32_t k = 0; k < nbatch; k++)
+		if ((int64_t) (b->h_offsets[k + 1] - b->h_offsets[k]) > maxrun)
+			maxrun = (int64_t) (b->h_offsets[k + 1] - b->h_offsets[k]);
+	CB_CUDA(ctx, cudaMallocAsync(&b->counts, (size_t) (maxrun + ninner + 1) * sizeof(unsigned long long), ctx->stream));
 	p.counts = b->counts;
 	if (p.f.ops && p.f.jointype != CB_JOIN_LEFT && maxrun)
 	{
@@ -1150,44 +1079,42 @@ ht_probe_batched(cbgpu_ctx *ctx, cbgpu_hashtable *ht, ProbeParams p, int fill_in
 		CB_CUDA(ctx, cudaMemsetAsync(b->matched, 0, (size_t) ninner, ctx->stream));
 		p.matched = b->matched;
 	}
-	/* HJ_NEED_NEW_BATCH (nodeHashjoin.c:709-738): each batch resident in turn, probed by its own run of outer rows */
+	if (iblocks > ctx->sm_count * 8)
+		iblocks = ctx->sm_count * 8;
 	for (int32_t batch = 0; batch < nbatch; batch++)
 	{
 		const int64_t m = (int64_t) (b->h_offsets[batch + 1] - b->h_offsets[batch]);
+		const int64_t nu = batch == nbatch - 1 ? ninner : 0;	/* build rows whose pairs follow this run's */
 		int			blocks = (int) ((m + 255) / 256);
 
-		if (interrupted && interrupted(arg))
-			return cb_fail(ctx, CBGPU_ERR_INTERRUPTED, "canceling statement due to user request%s", "");
-		if ((rc = cbgpu_ht_load_batch(ht, batch)) != CBGPU_OK)
-			return rc;
-		(*passes)++;
-		if (m == 0)
+		if (nbatch > 1)
+		{
+			if (interrupted && interrupted(arg))
+				return cb_fail(ctx, CBGPU_ERR_INTERRUPTED, "canceling statement due to user request%s", "");
+			if ((rc = cbgpu_ht_load_batch(ht, batch)) != CBGPU_OK)
+				return rc;
+			(*passes)++;
+			p.ht = ht->d;
+			p.sel = b->rows + b->h_offsets[batch];
+		}
+		if (m + nu == 0)
 			continue;
 		if (blocks > ctx->sm_count * 8)
 			blocks = ctx->sm_count * 8;
-		p.ht = ht->d;
-		p.sel = b->rows + b->h_offsets[batch];
 		p.n = m;
-		if ((rc = probe_pass(ctx, p, blocks, false)) != CBGPU_OK || (rc = pairs_append(ctx, b, &p, m, out, &any)) != CBGPU_OK)
+		p.ninner = nu;
+		if (m && (rc = probe_pass(ctx, p, blocks, false)) != CBGPU_OK)
 			return rc;
-		if (any && (rc = probe_pass(ctx, p, blocks, true)) != CBGPU_OK)
+		if (nu)
+		{
+			k_ht_unmatched_count<<<iblocks, 256, 0, ctx->stream>>>(p);
+			CB_LAUNCHED(ctx, "k_ht_unmatched_count");
+		}
+		if ((rc = pairs_append(ctx, b, &p, m + nu, out, &any)) != CBGPU_OK)
 			return rc;
-	}
-	if (ninner)
-	{
-		/* every pass has marked its matches: the build rows left unmatched come back once, behind all matched pairs */
-		int			iblocks = (int) ((ninner + 255) / 256);
-
-		if (iblocks > ctx->sm_count * 8)
-			iblocks = ctx->sm_count * 8;
-		p.sel = NULL;
-		p.n = 0;
-		p.ninner = ninner;
-		k_ht_unmatched_count<<<iblocks, 256, 0, ctx->stream>>>(p);
-		CB_LAUNCHED(ctx, "k_ht_unmatched_count");
-		if ((rc = pairs_append(ctx, b, &p, ninner, out, &any)) != CBGPU_OK)
+		if (any && m && (rc = probe_pass(ctx, p, blocks, true)) != CBGPU_OK)
 			return rc;
-		if (any)
+		if (any && nu)
 		{
 			k_ht_unmatched_write<<<iblocks, 256, 0, ctx->stream>>>(p);
 			CB_LAUNCHED(ctx, "k_ht_unmatched_write");
@@ -1196,32 +1123,31 @@ ht_probe_batched(cbgpu_ctx *ctx, cbgpu_hashtable *ht, ProbeParams p, int fill_in
 	return CBGPU_OK;
 }
 
-/* every pair probe: the resident table alone (nbatch <= 1) or batch by batch, with a join filter when `filter` is set.  On
- * failure *out is empty; the probe's own buffers are freed whatever the outcome. */
-static int
-ht_probe(cbgpu_ctx *ctx, cbgpu_hashtable *ht, cbgpu_rel *outer, const int32_t *keycols, int32_t nkeys, const uint32_t *sel,
-		 int64_t nsel, int left, int fill_inner, int32_t jointype, const cbgpu_join_filter *filter, int (*interrupted)(void *arg),
-		 void *arg, cbgpu_pairs *out, int64_t *passes)
+extern "C" int
+cbgpu_ht_probe_pairs(cbgpu_ctx *ctx, cbgpu_hashtable *ht, cbgpu_rel *outer, const int32_t *keycols, int32_t nkeys, int32_t jointype,
+					 const cbgpu_join_filter *filter, int (*interrupted)(void *arg), void *arg, cbgpu_pairs *out, int64_t *passes)
 {
-	BatchedProbe b;
+	const bool	taken = filter ? jointype == CB_JOIN_LEFT || jointype == CB_JOIN_SEMI || jointype == CB_JOIN_ANTI
+		: jointype == CB_JOIN_INNER || jointype == CB_JOIN_LEFT || jointype == CB_JOIN_RIGHT || jointype == CB_JOIN_FULL;
+	PairProbe	b;
 	ProbeParams p;
 	int64_t		npasses = 0;
 	int			rc;
 
 	memset(out, 0, sizeof(*out));
 	memset(&b, 0, sizeof(b));
-	rc = probe_params(ctx, ht, outer, keycols, nkeys, &p);
+	if (!taken)
+		rc = cb_fail(ctx, CBGPU_ERR_INVALID, "cbgpu_ht_probe_pairs: join type %s%lld (INNER, LEFT, RIGHT or FULL without a join "
+					 "filter, LEFT, SEMI or ANTI with one)", "", jointype);
+	else
+		rc = probe_params(ctx, ht, outer, keycols, nkeys, &p);
 	if (rc == CBGPU_OK && filter)
 		rc = join_filter_to_dev(ctx, filter, jointype, &b, &p.f);
 	if (rc == CBGPU_OK)
 	{
-		p.sel = sel;
-		p.n = sel ? nsel : outer->nrows;
-		p.left = left;
-		if (ht->d.nbatch > 1)
-			rc = ht_probe_batched(ctx, ht, p, fill_inner, interrupted, arg, &b, out, &npasses);
-		else
-			rc = ht_probe_single(ctx, ht, p, fill_inner, &b, out);
+		p.n = outer->nrows;
+		p.left = jointype == CB_JOIN_LEFT || jointype == CB_JOIN_FULL;
+		rc = ht_probe_batches(ctx, ht, p, jointype == CB_JOIN_RIGHT || jointype == CB_JOIN_FULL, interrupted, arg, &b, out, &npasses);
 	}
 	if (rc == CBGPU_OK && filter)
 		rc = cb_check_status(ctx, "join filter");	/* integer overflow inside the filter */
@@ -1241,65 +1167,6 @@ ht_probe(cbgpu_ctx *ctx, cbgpu_hashtable *ht, cbgpu_rel *outer, const int32_t *k
 	if (rc != CBGPU_OK)
 		cbgpu_pairs_free(out);
 	return rc;
-}
-
-/* the single-pass entry points: one pass sees the resident batch only, so the probe rows of every other batch would be missing */
-static int
-ht_probe_pairs(cbgpu_ctx *ctx, const cbgpu_hashtable *ht, cbgpu_rel *outer, const int32_t *keycols, int32_t nkeys,
-			   const uint32_t *sel, int64_t nsel, int left, int fill_inner, cbgpu_pairs *out)
-{
-	memset(out, 0, sizeof(*out));
-	if (ht->d.nbatch > 1)
-		return cb_fail(ctx, CBGPU_ERR_INVALID, "%sa table of %lld batches is probed for pairs by cbgpu_ht_probe_pairs_batched", "",
-					   ht->d.nbatch);
-	return ht_probe(ctx, (cbgpu_hashtable *) ht, outer, keycols, nkeys, sel, nsel, left, fill_inner, CB_JOIN_INNER, NULL, NULL,
-					NULL, out, NULL);
-}
-
-extern "C" int
-cbgpu_ht_probe_pairs_outer(cbgpu_ctx *ctx, const cbgpu_hashtable *ht, cbgpu_rel *outer, const int32_t *keycols, int32_t nkeys,
-						   int32_t fill_outer, int32_t fill_inner, cbgpu_pairs *out)
-{
-	return ht_probe_pairs(ctx, ht, outer, keycols, nkeys, NULL, 0, fill_outer != 0, fill_inner != 0, out);
-}
-
-extern "C" int
-cbgpu_ht_probe_pairs(cbgpu_ctx *ctx, const cbgpu_hashtable *ht, cbgpu_rel *outer, const int32_t *keycols, int32_t nkeys,
-					 const uint32_t *sel, int64_t nsel, cbgpu_pairs *out)
-{
-	return ht_probe_pairs(ctx, ht, outer, keycols, nkeys, sel, nsel, 0, 0, out);
-}
-
-extern "C" int
-cbgpu_ht_probe_pairs_left(cbgpu_ctx *ctx, const cbgpu_hashtable *ht, cbgpu_rel *outer, const int32_t *keycols, int32_t nkeys,
-						  cbgpu_pairs *out)
-{
-	return ht_probe_pairs(ctx, ht, outer, keycols, nkeys, NULL, 0, 1, 0, out);
-}
-
-extern "C" int
-cbgpu_ht_probe_pairs_batched(cbgpu_ctx *ctx, cbgpu_hashtable *ht, cbgpu_rel *outer, const int32_t *keycols, int32_t nkeys,
-							 int32_t fill_outer, int32_t fill_inner, int (*interrupted)(void *arg), void *arg, cbgpu_pairs *out,
-							 int64_t *passes)
-{
-	return ht_probe(ctx, ht, outer, keycols, nkeys, NULL, 0, fill_outer != 0, fill_inner != 0, CB_JOIN_INNER, NULL, interrupted,
-					arg, out, passes);
-}
-
-extern "C" int
-cbgpu_ht_probe_pairs_filtered(cbgpu_ctx *ctx, cbgpu_hashtable *ht, cbgpu_rel *outer, const int32_t *keycols, int32_t nkeys,
-							  int32_t jointype, const cbgpu_join_filter *filter, int (*interrupted)(void *arg), void *arg,
-							  cbgpu_pairs *out, int64_t *passes)
-{
-	memset(out, 0, sizeof(*out));
-	if (passes)
-		*passes = 0;
-	if (jointype != CB_JOIN_LEFT && jointype != CB_JOIN_SEMI && jointype != CB_JOIN_ANTI)
-		return cb_fail(ctx, CBGPU_ERR_INVALID, "cbgpu_ht_probe_pairs_filtered: join type %s%lld is not LEFT, SEMI or ANTI", "", jointype);
-	if (!filter)
-		return cb_fail(ctx, CBGPU_ERR_INVALID, "cbgpu_ht_probe_pairs_filtered: no join filter%s", "");
-	return ht_probe(ctx, ht, outer, keycols, nkeys, NULL, 0, jointype == CB_JOIN_LEFT, 0, jointype, filter, interrupted, arg, out,
-					passes);
 }
 
 extern "C" void

@@ -284,17 +284,14 @@ int			cbgpu_pipeline_run(cbgpu_ctx *ctx, const CbPipeline *p);
 /* ------------------------------------------------------------------------------------------
  * hash join tables
  * ------------------------------------------------------------------------------------------ */
-/* build over rows of `inner` (all rows, or those listed in sel[0..nsel)); key columns by index.
- * NULL keys are not inserted (strict hash operators, nodeHash.c:2161). */
-int			cbgpu_ht_build(cbgpu_ctx *ctx, cbgpu_rel *inner, const int32_t *keycols, int32_t nkeys,
+/* build over every row of `inner`; key columns by index.  NULL keys are not inserted (strict hash operators, nodeHash.c:2161).
+ * nbatch (a power of two up to 4096) above 1 makes a multi-batch hybrid hash join (nodeHash.c:980-990, 1133, 2223-2242):
+ * the build side is split into nbatch batches by bits of the key hash that the slot index does not use; the table holds
+ * one batch at a time (cbgpu_ht_load_batch) and sizes itself for the fullest.  A pipeline that probes it runs once per
+ * batch - probe rows of other batches are skipped in each pass - and its sink accumulates over the passes.
+ * cbgpu_ht_bytes_for(rows) = device bytes of a one-batch table, for choosing nbatch against a budget. */
+int			cbgpu_ht_build(cbgpu_ctx *ctx, cbgpu_rel *inner, const int32_t *keycols, int32_t nkeys, int32_t nbatch,
 						   cbgpu_hashtable **out);
-/* multi-batch hybrid hash join (nodeHash.c:980-990, 1133, 2223-2242): the build side is split into nbatch (a power of two)
- * batches by bits of the key hash that the slot index does not use; the table holds one batch at a time
- * (cbgpu_ht_load_batch) and sizes itself for the fullest.  A pipeline that probes it runs once per batch - probe rows of
- * other batches are skipped in each pass - and its sink accumulates over the passes.  cbgpu_ht_bytes_for(rows) = device
- * bytes of a one-batch table, for choosing nbatch against a budget. */
-int			cbgpu_ht_build_batched(cbgpu_ctx *ctx, cbgpu_rel *inner, const int32_t *keycols, int32_t nkeys, int32_t nbatch,
-								   cbgpu_hashtable **out);
 int			cbgpu_ht_nbatch(const cbgpu_hashtable *ht);
 int			cbgpu_ht_load_batch(cbgpu_hashtable *ht, int32_t batch);
 int64_t		cbgpu_ht_bytes_for(int64_t rows);
@@ -304,38 +301,13 @@ int			cbgpu_ht_has_duplicates(const cbgpu_hashtable *ht);
 /* the per-code hash table (device pointer) of dictionary key column k of the build side, NULL for other types:
  * the identity of the dictionary the build keys are coded by */
 const uint32_t *cbgpu_ht_key_dict_hash(const cbgpu_hashtable *ht, int32_t k);
-/* stand-alone probe emitting (outer_idx, inner_idx) pairs for an INNER join (all matches);
- * outer key columns by index.  pairs are written to two device arrays owned by the call result. */
+/* the result of a pair probe: (outer_idx, inner_idx) row-id pairs in two device arrays owned by the result */
 typedef struct cbgpu_pairs
 {
 	int64_t		npairs;
 	uint32_t   *outer_idx;		/* device                                                             */
 	uint32_t   *inner_idx;		/* device                                                             */
 } cbgpu_pairs;
-int			cbgpu_ht_probe_pairs(cbgpu_ctx *ctx, const cbgpu_hashtable *ht, cbgpu_rel *outer,
-								 const int32_t *keycols, int32_t nkeys, const uint32_t *sel, int64_t nsel,
-								 cbgpu_pairs *out);
-/* the same for a LEFT join: an outer row without a partner yields one pair whose inner_idx is 0xFFFFFFFF (a pipeline driven
- * by the pairs reads that source as NULL: HJ_FILL_OUTER_TUPLE, nodeHashjoin.c:640-660) */
-int			cbgpu_ht_probe_pairs_left(cbgpu_ctx *ctx, const cbgpu_hashtable *ht, cbgpu_rel *outer, const int32_t *keycols,
-									  int32_t nkeys, cbgpu_pairs *out);
-/* all outer-join flavours of the pair probe: fill_outer adds (row, 0xFFFFFFFF) for probe rows without a partner (LEFT /
- * FULL), fill_inner adds (0xFFFFFFFF, row) for build rows no probe row matched, NULL-keyed build rows included (RIGHT /
- * FULL: ExecScanHashTableForUnmatched nodeHash.c:2360, HJ_FILL_INNER_TUPLES nodeHashjoin.c:676-706) */
-int			cbgpu_ht_probe_pairs_outer(cbgpu_ctx *ctx, const cbgpu_hashtable *ht, cbgpu_rel *outer, const int32_t *keycols,
-									   int32_t nkeys, int32_t fill_outer, int32_t fill_inner, cbgpu_pairs *out);
-/* The three calls above probe the resident batch only, so they refuse a table of several batches (CBGPU_ERR_INVALID).
- * This one runs the whole join over such a table (ExecHashJoinImpl's HJ_NEED_NEW_BATCH loop, nodeHashjoin.c:709-738): every
- * row of `outer` is assigned to its key's batch once, then each batch is loaded in turn (0 .. nbatch - 1) and probed by its
- * own rows, and for fill_inner the build rows no batch matched come last.  fill_outer / fill_inner as in
- * cbgpu_ht_probe_pairs_outer; a NULL-keyed probe row belongs to batch 0.  Within one batch pairs are in outer-row order,
- * so the outer row ids come in the same order on every call (a row's partners in the table's slot order).  `interrupted` (may be NULL) is polled before each batch: nonzero stops the call with
- * CBGPU_ERR_INTERRUPTED.  *passes (may be NULL) = batches loaded and probed, also when the call fails.  On return the
- * table holds the last batch it loaded (nbatch - 1 after a success).  A one-batch table takes cbgpu_ht_probe_pairs_outer's
- * path with *passes = 0.  On failure *out is empty and nothing stays allocated. */
-int			cbgpu_ht_probe_pairs_batched(cbgpu_ctx *ctx, cbgpu_hashtable *ht, cbgpu_rel *outer, const int32_t *keycols,
-										 int32_t nkeys, int32_t fill_outer, int32_t fill_inner, int (*interrupted) (void *arg),
-										 void *arg, cbgpu_pairs *out, int64_t *passes);
 /* a join filter (the hash join's joinqual): a postfix program that must leave exactly one boolean.  Its columns address the
  * probe relation's row (src 0) or the build relation's row (src 1) of a key-equal candidate pair.  Ops: LOAD, CONST, DUP,
  * POP, integer and float8 arithmetic, I2F, F8ORD, the compares, AND / OR / NOT.  NULL or false: the pair does not match
@@ -347,19 +319,32 @@ typedef struct cbgpu_join_filter
 	int32_t		nops;
 	const CbpOp *ops;			/* host array                                                         */
 } cbgpu_join_filter;
-/* the pair probe of a LEFT, SEMI or ANTI hash join with a join filter: each key-equal candidate (ExecScanHashBucket,
- * nodeHash.c:2255) counts as a match only if `filter` passes for it (nodeHashjoin.c:583-713).  Pairs come in outer-row order
- * within each batch:
+/* the stand-alone pair probe of a hash join (N:M, or a join that returns unmatched rows); outer key columns by index.
+ * Without a join filter, jointype is
+ *   INNER: every match (ExecScanHashBucket walks the whole chain, nodeHash.c:2255);
+ *   LEFT: every match, and (row, 0xFFFFFFFF) for a probe row without a partner (a pipeline driven by the pairs reads that
+ *     source as NULL: HJ_FILL_OUTER_TUPLE, nodeHashjoin.c:640-660);
+ *   RIGHT: every match, and (0xFFFFFFFF, row) for a build row no probe row matched, NULL-keyed build rows included
+ *     (ExecScanHashTableForUnmatched nodeHash.c:2360, HJ_FILL_INNER_TUPLES nodeHashjoin.c:676-706);
+ *   FULL: both.
+ * With a join filter, each key-equal candidate counts as a match only if `filter` passes for it (nodeHashjoin.c:583-713),
+ * and jointype is
  *   SEMI: (row, first passing build row), at most one per row; NULL-keyed rows and rows with no passing candidate give none;
  *   ANTI: (row, 0xFFFFFFFF) for every row with no passing candidate, NULL-keyed rows included;
  *   LEFT: every passing pair, and (row, 0xFFFFFFFF) for a row with none.
- * A one-batch table and a table split into batches are both taken; batches, `interrupted`, *passes and the clean-up on
- * failure as in cbgpu_ht_probe_pairs_batched.  CBGPU_ERR_INVALID, before any launch, for another join type or a malformed
- * filter (a column src other than 0 / 1, a column or op outside the supported set, a stack deeper than CBP_STACK, a program
- * that does not leave exactly one value); CBGPU_ERR_OVERFLOW when the filter's integer arithmetic overflows on a pair. */
-int			cbgpu_ht_probe_pairs_filtered(cbgpu_ctx *ctx, cbgpu_hashtable *ht, cbgpu_rel *outer, const int32_t *keycols,
-										  int32_t nkeys, int32_t jointype, const cbgpu_join_filter *filter,
-										  int (*interrupted) (void *arg), void *arg, cbgpu_pairs *out, int64_t *passes);
+ * A table of several batches is probed batch by batch (ExecHashJoinImpl's HJ_NEED_NEW_BATCH loop, nodeHashjoin.c:709-738):
+ * every row of `outer` is assigned to its key's batch once (a NULL-keyed row to batch 0), then each batch is loaded in turn
+ * (0 .. nbatch - 1) and probed by its own rows.  Within one batch pairs are in outer-row order, so the outer row ids come in
+ * the same order on every call (a row's partners in the table's slot order); unmatched build rows come last.  `interrupted`
+ * (may be NULL) is polled before each batch of such a table: nonzero stops the call with CBGPU_ERR_INTERRUPTED.  *passes
+ * (may be NULL) = batches loaded and probed, 0 for a one-batch table, also when the call fails.  On return the table holds
+ * the last batch it loaded (nbatch - 1 after a success).  CBGPU_ERR_INVALID, before any launch, for a join type the call
+ * does not take with (or without) a filter, or a malformed filter (a column src other than 0 / 1, a column or op outside the
+ * supported set, a stack deeper than CBP_STACK, a program that does not leave exactly one value); CBGPU_ERR_OVERFLOW when
+ * the filter's integer arithmetic overflows on a pair.  On failure *out is empty and nothing stays allocated. */
+int			cbgpu_ht_probe_pairs(cbgpu_ctx *ctx, cbgpu_hashtable *ht, cbgpu_rel *outer, const int32_t *keycols, int32_t nkeys,
+								 int32_t jointype, const cbgpu_join_filter *filter, int (*interrupted) (void *arg), void *arg,
+								 cbgpu_pairs *out, int64_t *passes);
 void		cbgpu_pairs_free(cbgpu_pairs *p);
 int			cbgpu_read_u32(cbgpu_ctx *ctx, const uint32_t *dev, int64_t n, uint32_t *host);
 /* small device scratch (sink row counters, index vectors): zero-filled allocation, read-back, free */

@@ -82,11 +82,11 @@ def main():
     L = ctx.L
     keys = (C.c_int32 * 1)(0)
     ht = C.c_void_p()
-    ctx.check(L.cbgpu_ht_build_batched(ctx.h, inner.h, keys, 1, 16, C.byref(ht)))
+    ctx.check(L.cbgpu_ht_build(ctx.h, inner.h, keys, 1, 16, C.byref(ht)))
     pairs = capi.CbgpuPairs()
     passes = C.c_int64()
     before = ctx.launches()
-    ctx.check(L.cbgpu_ht_probe_pairs_batched(ctx.h, ht, outer.h, keys, 1, 1, 1, None, None, C.byref(pairs), C.byref(passes)))
+    ctx.check(L.cbgpu_ht_probe_pairs(ctx.h, ht, outer.h, keys, 1, P.JOIN_FULL, None, None, None, C.byref(pairs), C.byref(passes)))
     full = {"launches": ctx.launches() - before, "passes": passes.value}
     L.cbgpu_pairs_free(C.byref(pairs))
     polls = {"n": 0}
@@ -96,12 +96,11 @@ def main():
         return 1 if polls["n"] > 2 else 0
     cb = POLL(pending)
     before = ctx.launches()
-    rc = L.cbgpu_ht_probe_pairs_batched(ctx.h, ht, outer.h, keys, 1, 1, 1, C.cast(cb, C.c_void_p), None, C.byref(pairs), C.byref(passes))
+    rc = L.cbgpu_ht_probe_pairs(ctx.h, ht, outer.h, keys, 1, P.JOIN_FULL, None, C.cast(cb, C.c_void_p), None, C.byref(pairs),
+                                C.byref(passes))
     out["abi_interrupt"] = {"code": rc, "msg": ctx.error(), "launches": ctx.launches() - before, "passes": passes.value,
                             "polls": polls["n"], "npairs": pairs.npairs, "outer_idx": pairs.outer_idx, "full": full}
-    rc = L.cbgpu_ht_probe_pairs(ctx.h, ht, outer.h, keys, 1, None, 0, C.byref(pairs))
-    out["single_pass_refused"] = {"code": rc, "msg": ctx.error()}
-    ctx.check(L.cbgpu_ht_probe_pairs_batched(ctx.h, ht, outer.h, keys, 1, 0, 1, None, None, C.byref(pairs), C.byref(passes)))
+    ctx.check(L.cbgpu_ht_probe_pairs(ctx.h, ht, outer.h, keys, 1, P.JOIN_RIGHT, None, None, None, C.byref(pairs), C.byref(passes)))
     out["abi_after"] = {"passes": passes.value}
     L.cbgpu_pairs_free(C.byref(pairs))
     L.cbgpu_ht_free(ht)

@@ -1,6 +1,6 @@
-"""Worker of tests/test_host_join_filter_fake_runtime.py: the host side of the filtered pair probe (LEFT / SEMI / ANTI hash joins
-with a join filter) over tests/native/fake_cudart.c (LD_PRELOADed by the test; kernels are no-ops, "device" memory is zeroed
-host memory).  Prints one JSON object.  Not a test by itself."""
+"""Worker of tests/test_host_join_filter_fake_runtime.py: the host side of the pair probe (LEFT / SEMI / ANTI hash joins with a
+join filter, and INNER / FULL ones without) over tests/native/fake_cudart.c (LD_PRELOADed by the test; kernels are no-ops,
+"device" memory is zeroed host memory).  Prints one JSON object.  Not a test by itself."""
 import ctypes as C
 import json
 import os
@@ -63,13 +63,13 @@ def main():
     keys = (C.c_int32 * 1)(0)
     good = capi.join_filter([(outer, 1, 0), (inner, 1, 1)], [(capi.CBP_LOAD, 0, 0), (capi.CBP_LOAD, 1, 0), (capi.CBP_NE, 0, 0)])
     ht = C.c_void_p()
-    ctx.check(L.cbgpu_ht_build_batched(ctx.h, inner.h, keys, 1, 16, C.byref(ht)))
+    ctx.check(L.cbgpu_ht_build(ctx.h, inner.h, keys, 1, 16, C.byref(ht)))
     pairs, passes = capi.CbgpuPairs(), C.c_int64()
 
     def probe(filt, jointype=P.JOIN_SEMI, cb=None, table=ht):
         before = ctx.launches()
-        rc = L.cbgpu_ht_probe_pairs_filtered(ctx.h, table, outer.h, keys, 1, jointype, C.byref(filt) if filt is not None else None,
-                                             C.cast(cb, C.c_void_p) if cb else None, None, C.byref(pairs), C.byref(passes))
+        rc = L.cbgpu_ht_probe_pairs(ctx.h, table, outer.h, keys, 1, jointype, C.byref(filt) if filt is not None else None,
+                                    C.cast(cb, C.c_void_p) if cb else None, None, C.byref(pairs), C.byref(passes))
         r = {"code": rc, "msg": ctx.error() if rc else "", "launches": ctx.launches() - before, "passes": passes.value,
              "npairs": pairs.npairs, "outer_idx": pairs.outer_idx}
         L.cbgpu_pairs_free(C.byref(pairs))
@@ -92,9 +92,9 @@ def main():
         "bad_dup": capi.join_filter([], [(capi.CBP_DUP, 0, 0)]),
     }
     out["invalid"] = {k: probe(f) for k, f in bad.items()}
-    out["invalid"]["no_filter"] = probe(None)
+    out["invalid"]["no_filter"] = probe(None)                    # SEMI takes a filter
     for name, t in (("inner", P.JOIN_INNER), ("right", P.JOIN_RIGHT), ("full", P.JOIN_FULL), ("notin", P.JOIN_LASJ_NOTIN)):
-        out["invalid"]["jointype_" + name] = probe(good, t)
+        out["invalid"]["jointype_" + name] = probe(good, t)         # join types that take none
 
     # CHECK_FOR_INTERRUPTS between batches: the callback asks to stop when polled the third time
     polls = {"n": 0}
@@ -105,21 +105,22 @@ def main():
     cb = POLL(pending)
     out["abi_interrupt"] = dict(probe(good, P.JOIN_ANTI, cb), polls=polls["n"])
 
-    # every device allocation of the call failing in turn: CBGPU_ERR_NOMEM, nothing left behind, the next call clean
+    # every device allocation of the call failing in turn, with a filter and without: CBGPU_ERR_NOMEM, nothing left behind,
+    # the next call clean
     fake = C.CDLL(None)
     fake.fake_cudart_fail_alloc_in.argtypes = [C.c_long]
     oom = {"codes": [], "after": []}
-    for jointype in (P.JOIN_SEMI, P.JOIN_LEFT):
+    for jointype, filt in ((P.JOIN_SEMI, good), (P.JOIN_LEFT, good), (P.JOIN_INNER, None), (P.JOIN_FULL, None)):
         for batched in (True, False):
             table = ht
             if not batched:
                 table = C.c_void_p()
-                ctx.check(L.cbgpu_ht_build(ctx.h, inner.h, keys, 1, C.byref(table)))
+                ctx.check(L.cbgpu_ht_build(ctx.h, inner.h, keys, 1, 1, C.byref(table)))
             for n in range(1, 200):
                 fake.fake_cudart_fail_alloc_in(n)
-                r = probe(good, jointype, table=table)
+                r = probe(filt, jointype, table=table)
                 fake.fake_cudart_fail_alloc_in(0)
-                after = probe(good, jointype, table=table)
+                after = probe(filt, jointype, table=table)
                 oom["after"].append(after["code"])
                 if r["code"] == 0:
                     break

@@ -188,7 +188,7 @@ def _read_pairs(ctx, pairs, ordered=False):
     return (o, i) if ordered else sorted(zip(o.tolist(), i.tolist()))
 
 
-def test_pair_order_is_deterministic(ctx):
+def test_pair_order_of_the_batch_loop_is_deterministic(ctx):
     """the pair list comes out batch by batch, each batch's pairs in probe-row order, the unmatched build rows last: the same
     call twice gives the same probe-row sequence and the same pairs (the partners of one probe row come in the table's slot
     order, which each fill's concurrent inserts decide, as in the one-batch probe).  Rows of a query are a different matter:
@@ -199,13 +199,12 @@ def test_pair_order_is_deterministic(ctx):
     outer, inner = to_device(ctx, [fp, dp])
     keys = (C.c_int32 * 1)(0)
     ht = C.c_void_p()
-    ctx.check(L.cbgpu_ht_build_batched(ctx.h, inner.h, keys, 1, 32, C.byref(ht)))
+    ctx.check(L.cbgpu_ht_build(ctx.h, inner.h, keys, 1, 32, C.byref(ht)))
     pairs, passes = capi.CbgpuPairs(), C.c_int64()
-    for fill_outer, fill_inner in ((0, 0), (1, 1)):
+    for jointype, fill_inner in ((P.JOIN_INNER, False), (P.JOIN_FULL, True)):
         lists = []
         for _ in range(2):
-            ctx.check(L.cbgpu_ht_probe_pairs_batched(ctx.h, ht, outer.h, keys, 1, fill_outer, fill_inner, None, None, C.byref(pairs),
-                                                     C.byref(passes)))
+            ctx.check(L.cbgpu_ht_probe_pairs(ctx.h, ht, outer.h, keys, 1, jointype, None, None, None, C.byref(pairs), C.byref(passes)))
             lists.append(_read_pairs(ctx, pairs, ordered=True))
             L.cbgpu_pairs_free(C.byref(pairs))
         (o, i), (o2, i2) = lists
@@ -220,30 +219,26 @@ def test_pair_order_is_deterministic(ctx):
     inner.free()
 
 
-def test_abi_batched_pair_probe(ctx):
-    """cbgpu_ht_probe_pairs* refuse a multi-batch table (they would see one batch); cbgpu_ht_probe_pairs_batched over it
-    returns the pair set a one-batch table over the same rows gives, for every fill_outer / fill_inner flavour"""
+def test_abi_pair_probe_over_one_batch_and_sixteen(ctx):
+    """cbgpu_ht_probe_pairs over a 16-batch table returns the pair set a one-batch table over the same rows gives, for every
+    INNER / LEFT / RIGHT / FULL flavour"""
     L = ctx.L
     _, fp = make(fact, 20011, seed=91, null_frac=0.1, kmax=3000)
     _, dp = make(dim, 4000, seed=92, null_frac=0.1, dup=3, kmax=3000)
     outer, inner = to_device(ctx, [fp, dp])
     keys = (C.c_int32 * 1)(0)
     one, many = C.c_void_p(), C.c_void_p()
-    ctx.check(L.cbgpu_ht_build(ctx.h, inner.h, keys, 1, C.byref(one)))
-    ctx.check(L.cbgpu_ht_build_batched(ctx.h, inner.h, keys, 1, 16, C.byref(many)))
+    ctx.check(L.cbgpu_ht_build(ctx.h, inner.h, keys, 1, 1, C.byref(one)))
+    ctx.check(L.cbgpu_ht_build(ctx.h, inner.h, keys, 1, 16, C.byref(many)))
     assert L.cbgpu_ht_nbatch(one) == 1 and L.cbgpu_ht_nbatch(many) == 16
     pairs = capi.CbgpuPairs()
-    rc = L.cbgpu_ht_probe_pairs(ctx.h, many, outer.h, keys, 1, None, 0, C.byref(pairs))
-    assert rc == -2 and "cbgpu_ht_probe_pairs_batched" in ctx.error() and pairs.npairs == 0
-    for fill_outer, fill_inner in ((0, 0), (1, 0), (0, 1), (1, 1)):
-        rc = L.cbgpu_ht_probe_pairs_outer(ctx.h, many, outer.h, keys, 1, fill_outer, fill_inner, C.byref(pairs))
-        assert rc == -2 and pairs.npairs == 0
-        ctx.check(L.cbgpu_ht_probe_pairs_outer(ctx.h, one, outer.h, keys, 1, fill_outer, fill_inner, C.byref(pairs)))
+    for jointype in (P.JOIN_INNER, P.JOIN_LEFT, P.JOIN_RIGHT, P.JOIN_FULL):
+        passes = C.c_int64(-1)
+        ctx.check(L.cbgpu_ht_probe_pairs(ctx.h, one, outer.h, keys, 1, jointype, None, None, None, C.byref(pairs), C.byref(passes)))
         want = _read_pairs(ctx, pairs)
         L.cbgpu_pairs_free(C.byref(pairs))
-        passes = C.c_int64()
-        ctx.check(L.cbgpu_ht_probe_pairs_batched(ctx.h, many, outer.h, keys, 1, fill_outer, fill_inner, None, None, C.byref(pairs),
-                                                 C.byref(passes)))
+        assert passes.value == 0
+        ctx.check(L.cbgpu_ht_probe_pairs(ctx.h, many, outer.h, keys, 1, jointype, None, None, None, C.byref(pairs), C.byref(passes)))
         got = _read_pairs(ctx, pairs)
         L.cbgpu_pairs_free(C.byref(pairs))
         assert passes.value == 16 and got == want and len(want) > 20011

@@ -1,5 +1,5 @@
 """LEFT, SEMI and ANTI hash joins with a join filter (joinqual) on the GPU (-m gpu): the pair probe tests the filter on every
-key-equal candidate in its chain walk (cbgpu_ht_probe_pairs_filtered, k_ht_probe_filtered), SEMI / ANTI stop at the first
+key-equal candidate in its chain walk (cbgpu_ht_probe_pairs, k_ht_probe_filtered), SEMI / ANTI stop at the first
 passing candidate, and a LEFT row none of whose candidates pass is NULL-extended once (nodeHashjoin.c:583-713).  Every query
 is compared with the CPU oracle through both kernel routes, and the launch trace shows that the filtered probe ran.  Also:
 the plan's own qual on non-inner joins, the same joins split into batches at a 16 KB operator budget, overflow inside the
@@ -161,7 +161,7 @@ def test_duplicates_and_one_passing_candidate(ctx, oracle, dup, jointype, generi
 
 @pytest.mark.parametrize("nbatch", [1, 16])
 @pytest.mark.parametrize("jointype", JOINS)
-def test_the_passing_candidate_at_every_chain_position(ctx, oracle, jointype, nbatch):
+def test_filtered_pair_probe_finds_the_candidate_at_every_chain_position(ctx, oracle, jointype, nbatch):
     """all 600 build rows share one key and have distinct b; probe row r has a = r, so `o.a = i.b` lets exactly one candidate
     pass for each probe row, and over the 600 rows that candidate takes every position of the chain, the last one in slot order
     included.  SEMI must return each probe row with that one partner, ANTI none of them, LEFT one pair each."""
@@ -175,10 +175,10 @@ def test_the_passing_candidate_at_every_chain_position(ctx, oracle, jointype, nb
     keys = (C.c_int32 * 1)(0)
     filt = capi.join_filter([(outer, 1, 0), (inner, 1, 1)], [(capi.CBP_LOAD, 0, 0), (capi.CBP_LOAD, 1, 0), (capi.CBP_EQ, 0, 0)])
     ht = C.c_void_p()
-    ctx.check(L.cbgpu_ht_build_batched(ctx.h, inner.h, keys, 1, nbatch, C.byref(ht)))
+    ctx.check(L.cbgpu_ht_build(ctx.h, inner.h, keys, 1, nbatch, C.byref(ht)))
     pairs, passes = capi.CbgpuPairs(), C.c_int64()
-    ctx.check(L.cbgpu_ht_probe_pairs_filtered(ctx.h, ht, outer.h, keys, 1, jointype, C.byref(filt), None, None, C.byref(pairs),
-                                              C.byref(passes)))
+    ctx.check(L.cbgpu_ht_probe_pairs(ctx.h, ht, outer.h, keys, 1, jointype, C.byref(filt), None, None, C.byref(pairs),
+                                     C.byref(passes)))
     a, b = _read_pairs(ctx, pairs)
     L.cbgpu_pairs_free(C.byref(pairs))
     L.cbgpu_ht_free(ht)
@@ -285,8 +285,8 @@ def _brute(fo, do, jointype):
 
 
 @pytest.mark.parametrize("jointype", JOINS)
-def test_entry_point_against_a_nested_loop(ctx, jointype):
-    """cbgpu_ht_probe_pairs_filtered: pairs in outer-row order, at most one per row for SEMI / ANTI, the same pairs from a
+def test_pair_probe_against_a_nested_loop(ctx, jointype):
+    """cbgpu_ht_probe_pairs: pairs in outer-row order, at most one per row for SEMI / ANTI, the same pairs from a
     one-batch table and from the same build side split into 16 batches, and the pairs a nested loop gives"""
     L = ctx.L
     fo, fp = make(outer_rel, 6007, 71, 500)
@@ -298,10 +298,10 @@ def test_entry_point_against_a_nested_loop(ctx, jointype):
     results = []
     for nbatch in (1, 16):
         ht = C.c_void_p()
-        ctx.check(L.cbgpu_ht_build_batched(ctx.h, inner.h, keys, 1, nbatch, C.byref(ht)))
+        ctx.check(L.cbgpu_ht_build(ctx.h, inner.h, keys, 1, nbatch, C.byref(ht)))
         pairs, passes = capi.CbgpuPairs(), C.c_int64()
-        ctx.check(L.cbgpu_ht_probe_pairs_filtered(ctx.h, ht, outer.h, keys, 1, jointype, C.byref(filt), None, None, C.byref(pairs),
-                                                  C.byref(passes)))
+        ctx.check(L.cbgpu_ht_probe_pairs(ctx.h, ht, outer.h, keys, 1, jointype, C.byref(filt), None, None, C.byref(pairs),
+                                         C.byref(passes)))
         a, b = _read_pairs(ctx, pairs)
         L.cbgpu_pairs_free(C.byref(pairs))
         L.cbgpu_ht_free(ht)

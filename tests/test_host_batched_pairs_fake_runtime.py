@@ -3,8 +3,8 @@ libcbgpu.so over tests/native/fake_cudart.c, a CUDA runtime that computes nothin
 test_host_logic_fake_runtime.py does).  RIGHT and FULL joins at a 16 KB operator memory return no rows (no kernel computes
 anything) but walk every batch pass of the pair probe, the partition's read-back and the clean-up (INNER / LEFT ones run too,
 through the N:1 passes: a runtime that computes nothing reports no duplicate build keys); the interrupt
-callback stops the batch loop with CBGPU_ERR_INTERRUPTED; the single-pass pair probes refuse a multi-batch table.  Run as
-built and with libcbexec.so rebuilt under AddressSanitizer + UBSan."""
+callback stops the batch loop with CBGPU_ERR_INTERRUPTED.  Run as built and with libcbexec.so rebuilt under AddressSanitizer +
+UBSan."""
 import json
 import os
 import subprocess
@@ -16,7 +16,7 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 CUDA_INC = "/usr/local/cuda/include"
 pytestmark = pytest.mark.skipif(not os.path.exists(os.path.join(CUDA_INC, "cuda_runtime_api.h")), reason="needs the CUDA headers")
 
-INVALID, INTERRUPTED = -2, -8
+INTERRUPTED = -8
 
 
 @pytest.fixture(scope="module")
@@ -47,8 +47,6 @@ def _check(out):
     assert ai["launches"] < ai["full"]["launches"] and ai["full"]["passes"] == 16
     assert ai["npairs"] == 0 and ai["outer_idx"] is None         # a failed call leaves no pair list behind
     assert out["abi_after"]["passes"] == 16                       # and the table serves the next call
-    sr = out["single_pass_refused"]
-    assert sr["code"] == INVALID and "cbgpu_ht_probe_pairs_batched" in sr["msg"]
     ei = out["exec_interrupt"]
     assert ei["nbatch"] >= 4 and ei["polls_split"] - ei["polls_unsplit"] >= ei["nbatch"]
     assert set(ei["codes"]) == {INTERRUPTED} and len(ei["codes"]) == ei["polls_split"]
@@ -56,12 +54,12 @@ def _check(out):
     assert ei["rows_after"] == [0] * len(ei["codes"])
 
 
-def test_batched_pair_joins_over_a_runtime_that_computes_nothing(fake):
+def test_pair_joins_in_batches_over_a_runtime_that_computes_nothing(fake):
     _, so = fake
     _check(_run({"LD_PRELOAD": so}))
 
 
-def test_the_same_under_address_and_ub_sanitizers(fake):
+def test_pair_joins_in_batches_under_address_and_ub_sanitizers(fake):
     d, so = fake
     asan = subprocess.check_output(["gcc", "-print-file-name=libasan.so"], text=True).strip()
     if not os.path.exists(asan):

@@ -1,9 +1,10 @@
 """The host side of LEFT / SEMI / ANTI hash joins with a join filter, without a GPU (not gpu): libcbexec.so + the host code of
 libcbgpu.so over tests/native/fake_cudart.c, a CUDA runtime that computes nothing (LD_PRELOADed into a subprocess, as
 test_host_batched_pairs_fake_runtime.py does).  The filtered joins run to zero rows with launches, at 16 KB in batches; RIGHT,
-FULL and NOT IN joins with a join filter are still refused; cbgpu_ht_probe_pairs_filtered refuses every malformed filter and
-other join types before any launch, stops between batches when interrupted, and reports CBGPU_ERR_NOMEM for each of its
-device allocations failing in turn, with the next call clean.  Run as built and with libcbexec.so rebuilt under
+FULL and NOT IN joins with a join filter are still refused; cbgpu_ht_probe_pairs refuses every malformed filter, a filter on
+a join type that takes none and a SEMI join without one before any launch, stops between batches when interrupted, and
+reports CBGPU_ERR_NOMEM for each of its device allocations failing in turn (filtered and unfiltered, one batch and 16), with
+the next call clean.  Run as built and with libcbexec.so rebuilt under
 AddressSanitizer + UBSan."""
 import json
 import os
@@ -63,12 +64,12 @@ def _check(out):
     assert set(oom["after"]) == {0}, oom
 
 
-def test_filtered_pair_joins_over_a_runtime_that_computes_nothing(fake):
+def test_pair_probe_with_and_without_filters_over_a_runtime_that_computes_nothing(fake):
     _, so = fake
     _check(_run({"LD_PRELOAD": so}))
 
 
-def test_the_same_under_address_and_ub_sanitizers(fake):
+def test_pair_probe_with_and_without_filters_under_address_and_ub_sanitizers(fake):
     d, so = fake
     asan = subprocess.check_output(["gcc", "-print-file-name=libasan.so"], text=True).strip()
     if not os.path.exists(asan):
