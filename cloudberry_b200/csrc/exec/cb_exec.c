@@ -573,44 +573,173 @@ stream_new(NodePriv *p)
 	return s;
 }
 
-/* identity stream over a relation whose columns follow `shape` (column layout of a materialised
- * stream: one column per scalar output, three per transition state) */
+/*
+ * The column layout of a stream's rows stored as a relation (a materialised stream, a Motion's send and receive buffers, a
+ * Hash node's build side): `lead` leading columns first (a hash Motion's key values), then one column per scalar output and
+ * three per transition state (N, sum.lo, sum.hi).  colstart[i] (when given) gets the first column of output i; returns the
+ * number of columns.
+ */
 static int
-stream_over_rel(CbEState *es, CbStream *s, cbgpu_rel *rel, const PExpr *shape, int nshape)
+shape_columns(const PExpr *shape, int n, int lead, int *colstart)
 {
-	int			c = 0;
+	int			c = lead;
+
+	for (int i = 0; i < n; i++)
+	{
+		if (colstart)
+			colstart[i] = c;
+		c += shape[i].kind == PE_STATE ? 3 : 1;
+	}
+	return c;
+}
+
+/* the sink columns a stream's rows are written to, in the layout of shape_columns */
+typedef struct SinkLayout
+{
+	int			ncols;
+	int32_t		types[CBP_MAX_OUT];
+	int32_t		dscales[CBP_MAX_OUT];
+	int			nullable[CBP_MAX_OUT];
+} SinkLayout;
+
+/* output expressions reading the outputs of `shape` from a relation: output i from column colstart[i] (N / lo / hi from there
+ * for a transition state), as source `src` of the pipeline; `nullable`: every value may be NULL (the missing side of an
+ * outer join) */
+static int
+pe_outputs_over_rel(CbEState *es, CbStream *s, cbgpu_rel *rel, const PExpr *shape, int n, const int *colstart, int src,
+					int nullable, int *out)
+{
+	for (int i = 0; i < n; i++)
+	{
+		const int	c = colstart[i];
+
+		if (shape[i].kind == PE_STATE)
+		{
+			PExpr		e = shape[i];
+
+			e.cn = pe_col(s, rel, c, src, nullable);
+			e.clo = pe_col(s, rel, c + 1, src, nullable);
+			e.chi = pe_col(s, rel, c + 2, src, nullable);
+			out[i] = (e.cn < 0 || e.clo < 0 || e.chi < 0) ? -1 : pe_add(s, &e);
+		}
+		else
+		{
+			out[i] = pe_col(s, rel, c, src, nullable);
+			if (out[i] >= 0)
+			{
+				/* keep the logical type / scale of the producing expression */
+				s->pe[out[i]].dscale = shape[i].dscale;
+			}
+		}
+		if (out[i] < 0)
+			return es_fail(es, CBGPU_ERR_UNSUPPORTED, "too many columns in one pipeline");
+	}
+	return CBGPU_OK;
+}
+
+/* identity stream over a relation whose columns follow `shape` after `lead` leading columns (shape_columns) */
+static int
+stream_over_rel(CbEState *es, CbStream *s, cbgpu_rel *rel, const PExpr *shape, int nshape, int lead)
+{
+	int			colstart[MAX_OUT];
 
 	s->pipe.nrows = cbgpu_rel_nrows(rel);
 	s->rows_in = s->pipe.nrows;
 	s->nsrc = 1;
 	s->nout = nshape;
-	for (int i = 0; i < nshape; i++)
-	{
-		if (shape[i].kind == PE_STATE)
-		{
-			PExpr		e = shape[i];
+	shape_columns(shape, nshape, lead, colstart);
+	return pe_outputs_over_rel(es, s, rel, shape, nshape, colstart, 0, 0, s->out);
+}
 
-			e.cn = pe_col(s, rel, c, 0, 0);
-			e.clo = pe_col(s, rel, c + 1, 0, 0);
-			e.chi = pe_col(s, rel, c + 2, 0, 0);
-			if (e.cn < 0 || e.clo < 0 || e.chi < 0)
-				return es_fail(es, CBGPU_ERR_UNSUPPORTED, "too many columns in one pipeline");
-			s->out[i] = pe_add(s, &e);
-			c += 3;
+/* emit the program tail that writes the values of the `nlead` leading (scalar) expressions, then the stream's outputs, as
+ * sink columns laid out by shape_columns; *lay gets those columns and shape[] the outputs' expressions */
+static int
+emit_sink_columns(CbEState *es, CbStream *s, const int *lead, int nlead, SinkLayout *lay, PExpr *shape)
+{
+	for (int i = 0; i < s->nout; i++)
+		shape[i] = s->pe[s->out[i]];
+	if (shape_columns(shape, s->nout, nlead, NULL) > CBP_MAX_OUT)
+		return es_fail(es, CBGPU_ERR_UNSUPPORTED, "too many output columns for one pipeline");
+	lay->ncols = 0;
+	for (int i = 0; i < nlead + s->nout; i++)
+	{
+		const int	e = i < nlead ? lead[i] : s->out[i - nlead];
+		const PExpr *x = &s->pe[e];
+
+		if (x->kind == PE_STATE)
+		{
+			const int	part[3] = {x->cn, x->clo, x->chi};
+
+			for (int k = 0; k < 3; k++)
+			{
+				lay->types[lay->ncols] = CB_INT8;
+				lay->dscales[lay->ncols] = 0;
+				lay->nullable[lay->ncols] = 0;
+				lay->ncols++;
+				TRY(emit_expr(es, s, part[k]));
+			}
 		}
 		else
 		{
-			s->out[i] = pe_col(s, rel, c, 0, 0);
-			if (s->out[i] >= 0)
-			{
-				/* keep the logical type / scale of the producing expression */
-				s->pe[s->out[i]].dscale = shape[i].dscale;
-			}
-			c += 1;
+			lay->types[lay->ncols] = x->type;
+			lay->dscales[lay->ncols] = x->dscale;
+			lay->nullable[lay->ncols] = x->maybe_null;
+			lay->ncols++;
+			TRY(emit_expr(es, s, e));
 		}
-		if (s->out[i] < 0)
-			return es_fail(es, CBGPU_ERR_UNSUPPORTED, "too many columns in one pipeline");
 	}
+	return emit_op(es, s, CBP_END, 0, 0);
+}
+
+/* a relation of `nrows` rows for the sink columns `lay`, owned by `own` */
+static int
+rel_create_for_sink(CbEState *es, Owned *own, const SinkLayout *lay, int64_t nrows, cbgpu_rel **out)
+{
+	GPU(es, cbgpu_rel_create(es->es_ctx, nrows, lay->ncols, lay->types, lay->dscales, out));
+	own->rels[own->nrels++] = *out;
+	for (int c = 0; c < lay->ncols; c++)
+		if (lay->nullable[c])
+			GPU(es, cbgpu_rel_add_nullmap(*out, c));
+	return CBGPU_OK;
+}
+
+/* dictionary columns keep their per-code hashes so they stay usable as join, group and Motion keys: share them into `rel`,
+ * whose columns hold the `nlead` leading expressions and then the outputs `shape` of stream `s` (emit_sink_columns) */
+static int
+rel_share_dicts(CbEState *es, cbgpu_rel *rel, const CbStream *s, const int *lead, int nlead, const PExpr *shape, int n)
+{
+	int			colstart[MAX_OUT];
+
+	shape_columns(shape, n, nlead, colstart);
+	for (int i = 0; i < nlead + n; i++)
+	{
+		const PExpr *x = i < nlead ? &s->pe[lead[i]] : &shape[i - nlead];
+		const int	c = i < nlead ? i : colstart[i - nlead];
+
+		if (x->kind == PE_COL && (x->type == CB_DICT8 || x->type == CB_DICT32) && s->pipe.cols[x->col].dict_hash)
+			GPU(es, cbgpu_rel_share_dict_hash(rel, c, s->col_rel[x->col], s->col_idx[x->col]));
+	}
+	return CBGPU_OK;
+}
+
+/* a relation of `nrows` rows with the column types, scales and dictionaries of `like`, owned by `own` */
+static int
+rel_create_like(CbEState *es, Owned *own, const cbgpu_rel *like, int64_t nrows, cbgpu_rel **out)
+{
+	int32_t		types[CBP_MAX_OUT],
+				dscales[CBP_MAX_OUT];
+	const int	ncols = cbgpu_rel_ncols(like);
+
+	for (int c = 0; c < ncols; c++)
+	{
+		types[c] = cbgpu_rel_col_type(like, c);
+		dscales[c] = cbgpu_rel_col_dscale(like, c);
+	}
+	GPU(es, cbgpu_rel_create(es->es_ctx, nrows, ncols, types, dscales, out));
+	own->rels[own->nrels++] = *out;
+	for (int c = 0; c < ncols; c++)
+		if (cbgpu_rel_dict_hash_dev(like, c))
+			GPU(es, cbgpu_rel_share_dict_hash(*out, c, like, c));
 	return CBGPU_OK;
 }
 
@@ -694,122 +823,72 @@ cbgpu_rel_is_base(const CbEState *es, const cbgpu_rel *rel)
 	return 0;
 }
 
+/* is PE e column c of the stream's relation? */
+static int
+pe_is_rel_col(const CbStream *s, int e, int c)
+{
+	return s->pe[e].kind == PE_COL && s->col_idx[s->pe[e].col] == c;
+}
+
+/* does the plain stream (stream_is_plain) expose `rel` column for column, in the layout of shape_columns?  shape[] gets the
+ * stream's outputs either way */
+static int
+stream_is_rel_layout(const CbStream *s, const cbgpu_rel *rel, PExpr *shape)
+{
+	int			colstart[MAX_OUT];
+
+	for (int i = 0; i < s->nout; i++)
+		shape[i] = s->pe[s->out[i]];
+	if (shape_columns(shape, s->nout, 0, colstart) != cbgpu_rel_ncols(rel))
+		return 0;
+	for (int i = 0; i < s->nout; i++)
+	{
+		const PExpr *x = &shape[i];
+		const int	c = colstart[i];
+
+		if (x->kind == PE_STATE ? !(pe_is_rel_col(s, x->cn, c) && pe_is_rel_col(s, x->clo, c + 1) && pe_is_rel_col(s, x->chi, c + 2)) :
+			!pe_is_rel_col(s, s->out[i], c))
+			return 0;
+	}
+	return 1;
+}
+
 /* run the stream into a new relation (MATERIALIZE sink); columns laid out as stream_over_rel expects */
 static int
 stream_materialize_ex(CbEState *es, CbPlanState *ps, CbStream *s, Owned *own, cbgpu_rel **out, PExpr *shape, int *nshape, int borrow)
 {
-	int32_t		types[CBP_MAX_OUT],
-				dscales[CBP_MAX_OUT];
-	int			ncols = 0;
-	int			nullable[CBP_MAX_OUT];
+	SinkLayout	lay;
 	cbgpu_rel  *rel;
 	void	   *counter;
 	int64_t		count = 0;
 	CbPipeline *p = &s->pipe;
 	int			saved_nops = p->nops;
 
-	if (borrow && stream_is_plain(s, &rel, NULL))
+	if (borrow && stream_is_plain(s, &rel, NULL) && stream_is_rel_layout(s, rel, shape) && !cbgpu_rel_is_base(es, rel))
 	{
 		/* the stream already IS a relation with exactly these columns (an aggregate's group relation, a Motion's receive
 		 * buffer): hand it over instead of copying it through a kernel.  The caller does not own it - its producer does. */
-		int			exact = 1,
-					c = 0;
+		int			mine = borrow != 2;
 
-		for (int i = 0; i < s->nout && exact; i++)
-		{
-			PExpr	   *x = &s->pe[s->out[i]];
-
-			shape[i] = *x;
-			if (x->kind == PE_STATE)
-			{
-				if (s->pe[x->cn].kind != PE_COL || s->col_idx[s->pe[x->cn].col] != c || s->pe[x->clo].kind != PE_COL ||
-					s->col_idx[s->pe[x->clo].col] != c + 1 || s->pe[x->chi].kind != PE_COL || s->col_idx[s->pe[x->chi].col] != c + 2)
-					exact = 0;
-				c += 3;
-			}
-			else
-			{
-				if (x->kind != PE_COL || s->col_idx[x->col] != c)
-					exact = 0;
-				c++;
-			}
-		}
-		if (exact && c == cbgpu_rel_ncols(rel) && !cbgpu_rel_is_base(es, rel) && borrow == 2)
-		{
-			/* the caller takes the relation over: only if it is this node's own */
-			exact = 0;
-			for (int i = 0; i < own->nrels; i++)
-				if (own->rels[i] == rel)
-					exact = 1;
-		}
-		if (exact && c == cbgpu_rel_ncols(rel) && !cbgpu_rel_is_base(es, rel))
+		/* the caller takes the relation over: only if it is this node's own */
+		for (int i = 0; i < own->nrels && !mine; i++)
+			mine = own->rels[i] == rel;
+		if (mine)
 		{
 			*nshape = s->nout;
 			*out = rel;
 			return CBGPU_OK;
 		}
 	}
-	for (int i = 0; i < s->nout; i++)
-	{
-		PExpr	   *x = &s->pe[s->out[i]];
-
-		shape[i] = *x;
-		if (x->kind == PE_STATE)
-		{
-			if (ncols + 3 > CBP_MAX_OUT)
-				return es_fail(es, CBGPU_ERR_UNSUPPORTED, "too many output columns for one pipeline");
-			for (int k = 0; k < 3; k++)
-			{
-				types[ncols] = CB_INT8;
-				dscales[ncols] = 0;
-				nullable[ncols] = 0;
-				ncols++;
-			}
-			TRY(emit_expr(es, s, x->cn));
-			TRY(emit_expr(es, s, x->clo));
-			TRY(emit_expr(es, s, x->chi));
-		}
-		else
-		{
-			if (ncols + 1 > CBP_MAX_OUT)
-				return es_fail(es, CBGPU_ERR_UNSUPPORTED, "too many output columns for one pipeline");
-			types[ncols] = x->type == CB_BOOL ? CB_BOOL : x->type;
-			dscales[ncols] = x->dscale;
-			nullable[ncols] = x->maybe_null;
-			ncols++;
-			TRY(emit_expr(es, s, s->out[i]));
-		}
-	}
+	TRY(emit_sink_columns(es, s, NULL, 0, &lay, shape));
 	*nshape = s->nout;
-	TRY(emit_op(es, s, CBP_END, 0, 0));
-	GPU(es, cbgpu_rel_create(es->es_ctx, p->nrows, ncols, types, dscales, &rel));
-	own->rels[own->nrels++] = rel;
-	for (int c = 0; c < ncols; c++)
-		if (nullable[c])
-			GPU(es, cbgpu_rel_add_nullmap(rel, c));
-	/* dictionary columns keep their per-code hashes so they stay usable as hash keys */
-	{
-		int			c = 0;
-
-		for (int i = 0; i < s->nout; i++)
-		{
-			PExpr	   *x = &s->pe[s->out[i]];
-
-			if (x->kind == PE_STATE)
-			{
-				c += 3;
-				continue;
-			}
-			if (x->kind == PE_COL && (x->type == CB_DICT8 || x->type == CB_DICT32) && p->cols[x->col].dict_hash)
-				GPU(es, cbgpu_rel_share_dict_hash(rel, c, s->col_rel[x->col], s->col_idx[x->col]));
-			c++;
-		}
-	}
+	TRY(rel_create_for_sink(es, own, &lay, p->nrows, &rel));
+	TRY(rel_share_dicts(es, rel, s, NULL, 0, shape, s->nout));
 	GPU(es, cbgpu_dev_alloc(es->es_ctx, sizeof(int64_t), &counter));
 	own->devs[own->ndevs++] = counter;
 	memset(&p->sink, 0, sizeof(p->sink));
 	p->sink.kind = CBP_SINK_MATERIALIZE;
-	p->sink.nout = ncols;
+	p->sink.nout = lay.ncols;
 	p->sink.out = rel;
 	p->sink.out_count = (int64_t *) counter;
 	p->force_generic = es->es_force_generic;
@@ -938,15 +1017,10 @@ hash_build(CbPlanState *hashps)
 	}
 	if (!rel)
 	{
-		int			n,
-					c = 0;
+		int			n;
 
 		TRY(stream_materialize(es, hashps, is, &p->owned, &rel, p->inner_pe, &n));
-		for (int i = 0; i < n; i++)
-		{
-			p->inner_map[i] = c;
-			c += p->inner_pe[i].kind == PE_STATE ? 3 : 1;
-		}
+		shape_columns(p->inner_pe, n, 0, p->inner_map);
 	}
 	for (int k = 0; k < h->nhashkeys; k++)
 	{
@@ -972,32 +1046,6 @@ hash_build(CbPlanState *hashps)
 	p->inner_rel = rel;
 	hashps->instrument.kernels += cbgpu_kernel_launches(es->es_ctx) - before;
 	hashps->instrument.ntuples = (double) cbgpu_ht_nrows(p->ht);
-	return CBGPU_OK;
-}
-
-static int
-inner_out_exprs(CbEState *es, CbStream *s, NodePriv *hp, int src, int nullable, int *inner)
-{
-	for (int i = 0; i < hp->inner_nout; i++)
-	{
-		if (hp->inner_pe[i].kind == PE_STATE)
-		{
-			PExpr		e = hp->inner_pe[i];
-
-			e.cn = pe_col(s, hp->inner_rel, hp->inner_map[i], src, nullable);
-			e.clo = pe_col(s, hp->inner_rel, hp->inner_map[i] + 1, src, nullable);
-			e.chi = pe_col(s, hp->inner_rel, hp->inner_map[i] + 2, src, nullable);
-			inner[i] = pe_add(s, &e);
-		}
-		else
-		{
-			inner[i] = pe_col(s, hp->inner_rel, hp->inner_map[i], src, nullable);
-			if (inner[i] >= 0)
-				s->pe[inner[i]].dscale = hp->inner_pe[i].dscale;
-		}
-		if (inner[i] < 0)
-			return es_fail(es, CBGPU_ERR_UNSUPPORTED, "too many columns in one pipeline");
-	}
 	return CBGPU_OK;
 }
 
@@ -1048,16 +1096,17 @@ static int
 join_filter_program(CbEState *es, CbStream *fs, cbgpu_rel *orel, const PExpr *shape, int nouter, NodePriv *hp, const CbHashJoin *hj)
 {
 	int			fouter[MAX_OUT],
-				finner[MAX_OUT];
+				finner[MAX_OUT],
+				colstart[MAX_OUT];
 	uint8_t		used[2][MAX_OUT];
-	int			e = -1,
-				c = 0;
+	int			e = -1;
 	VarCtx		vc;
 
 	/* only the columns the filter reads go into its column table (and to the device) */
 	memset(used, 0, sizeof(used));
 	for (int i = 0; i < hj->njoinquals; i++)
 		filter_vars_used(hj->joinqual[i], used);
+	shape_columns(shape, nouter, 0, colstart);
 	for (int i = 0; i < nouter; i++)
 	{
 		fouter[i] = -1;
@@ -1065,11 +1114,10 @@ join_filter_program(CbEState *es, CbStream *fs, cbgpu_rel *orel, const PExpr *sh
 		{
 			if (shape[i].kind == PE_STATE)
 				return es_fail(es, CBGPU_ERR_UNSUPPORTED, "join filter over an aggregate transition state is not supported on the GPU path");
-			if ((fouter[i] = pe_col(fs, orel, c, 0, 0)) < 0)
+			if ((fouter[i] = pe_col(fs, orel, colstart[i], 0, 0)) < 0)
 				return es_fail(es, CBGPU_ERR_UNSUPPORTED, "too many columns in one join filter");
 			fs->pe[fouter[i]].dscale = shape[i].dscale;
 		}
-		c += shape[i].kind == PE_STATE ? 3 : 1;
 	}
 	for (int i = 0; i < hp->inner_nout; i++)
 	{
@@ -1164,7 +1212,7 @@ open_hashjoin(CbPlanState *ps, CbStream **out)
 		cbgpu_join_filter jf;
 		int64_t		passes = 0;
 		NodePriv   *me = np(ps);
-		int			c,
+		int			colstart[MAX_OUT],
 					rc;
 
 		/* append the key expressions as extra output columns so the probe can read them */
@@ -1175,11 +1223,9 @@ open_hashjoin(CbPlanState *ps, CbStream **out)
 			s->out[s->nout++] = keys[k];
 		}
 		TRY(stream_materialize(es, ps, s, &me->owned, &orel, shape, &nshape));
-		c = 0;
-		for (int i = 0; i < nouter; i++)
-			c += shape[i].kind == PE_STATE ? 3 : 1;
+		shape_columns(shape, nshape, 0, colstart);
 		for (int k = 0; k < hj->nhashkeys; k++)
-			keycols[k] = c + k;
+			keycols[k] = colstart[nouter + k];
 		if (me->owned.npairs >= 8)
 			return es_fail(es, CBGPU_ERR_UNSUPPORTED, "too many N:M joins under one node");
 		pairs = &me->owned.pairs[me->owned.npairs++];
@@ -1204,7 +1250,7 @@ open_hashjoin(CbPlanState *ps, CbStream **out)
 		if (rc != CBGPU_OK)
 			return es_fail(es, rc, "%s", cbgpu_last_error(es->es_ctx));
 		s2 = stream_new(me);
-		TRY(stream_over_rel(es, s2, orel, shape, nouter));
+		TRY(stream_over_rel(es, s2, orel, shape, nouter, 0));
 		if (fill_inner)
 			for (int i = 0; i < s2->npe; i++)
 				s2->pe[i].maybe_null = 1;	/* the outer side of an unmatched build row is NULL */
@@ -1220,7 +1266,7 @@ open_hashjoin(CbPlanState *ps, CbStream **out)
 			for (int i = 0; i < hp->inner_nout; i++)
 				inner[i] = -1;	/* no inner columns survive a semi / anti join */
 		else
-			TRY(inner_out_exprs(es, s2, hp, 1, fill_outer, inner));
+			TRY(pe_outputs_over_rel(es, s2, hp->inner_rel, hp->inner_pe, hp->inner_nout, hp->inner_map, 1, fill_outer, inner));
 		s = s2;
 		vc.s = s;
 	}
@@ -1290,7 +1336,8 @@ open_hashjoin(CbPlanState *ps, CbStream **out)
 				inner[i] = -1;
 		}
 		else
-			TRY(inner_out_exprs(es, s, hp, base + j, hj->jointype == CB_JOIN_LEFT, inner));
+			TRY(pe_outputs_over_rel(es, s, hp->inner_rel, hp->inner_pe, hp->inner_nout, hp->inner_map, base + j,
+									hj->jointype == CB_JOIN_LEFT, inner));
 	}
 	vc.outer = outer;
 	vc.nouter = nouter;
@@ -2272,13 +2319,8 @@ open_agg(CbPlanState *ps, CbStream **out)
 		GPU(es, cbgpu_agg_to_rel(t, keytypes, &rel));
 		p->owned.rels[p->owned.nrels++] = rel;
 	}
-	for (int k = 0; k < info.nkeys; k++)
-	{
-		PExpr	   *kx = &cs->pe[info.keys[k]];
-
-		if ((kx->type == CB_DICT8 || kx->type == CB_DICT32) && kx->kind == PE_COL)
-			GPU(es, cbgpu_rel_share_dict_hash(rel, k, cs->col_rel[kx->col], cs->col_idx[kx->col]));
-	}
+	/* the grouping keys lead the groups' relation */
+	TRY(rel_share_dicts(es, rel, cs, info.keys, info.nkeys, NULL, 0));
 	s = stream_new(p);
 	s->pipe.nrows = cbgpu_rel_nrows(rel);
 	s->rows_in = s->pipe.nrows;
@@ -2353,6 +2395,166 @@ partition_pass(CbPlanState *ps, CbStream *s, cbgpu_rel *out, void *counter, void
 	return CBGPU_OK;
 }
 
+/* direct Motion (interconnects with peer memory): the PARTITION sink stores every row straight into its destination
+ * segment's receive window - no send buffer, no separate exchange, no collective.  Sets *delivered (and np(ps)->recv) when
+ * the rows were delivered; leaves the Motion to motion_send_staged when the interconnect has no direct path or asks for a
+ * retry. */
+static int
+motion_send_direct(CbPlanState *ps, CbStream *s, const SinkLayout *lay, void *counter, int64_t *counts, cbgpu_rel **send,
+				   int *delivered)
+{
+	CbEState   *es = ps->state;
+	CbMotion   *m = (CbMotion *) ps->plan;
+	NodePriv   *p = np(ps);
+	CbPipeline *pl = &s->pipe;
+	CbInterconnect *ic = es->es_cluster ? NULL : es->es_interconnect;
+	cbgpu_direct_dest dest;
+	cbgpu_rel  *rel,
+			   *recv = NULL;
+	int32_t		outcome = CBGPU_DX_DELIVERED;
+	uint64_t	nullmask = 0;
+	int			rc,
+				rc2;
+	int64_t		before;
+
+	for (int c = 0; c < lay->ncols; c++)
+		if (lay->nullable[c])
+			nullmask |= 1ull << c;
+	if (!ic || !ic->direct_begin || ic->direct_begin(ic, es, m->motionID, lay->ncols, lay->types, lay->dscales, &dest) != CBGPU_OK)
+		return CBGPU_OK;
+	before = cbgpu_kernel_launches(es->es_ctx);
+	/* from here to direct_end nothing may return early: the peers wait for this segment's signal */
+	rc = cbgpu_rel_create(es->es_ctx, 0, lay->ncols, lay->types, lay->dscales, &rel);
+	if (rc == CBGPU_OK)
+	{
+		p->owned.rels[p->owned.nrels++] = rel;
+		pl->sink.out = rel;
+		pl->sink.seg_capacity = dest.capacity;
+		pl->sink.part_cols = dest.cols;
+		pl->sink.part_counts = dest.counts;
+		pl->sink.part_nulls = dest.nulls;
+		pl->sink.part_nullmask = nullmask;
+		pl->sink.part_flags = dest.flags;
+		rc = run_pipeline(es, pl);
+	}
+	if (rc && es->es_errcode == 0)
+		es_fail(es, rc, "%s", cbgpu_last_error(es->es_ctx));
+	rc2 = ic->direct_end(ic, es, m->motionID, rc ? CBGPU_DX_ERROR : 0, nullmask, (const int64_t *) counter, counts, &recv, &outcome);
+	p->xstage = 1;
+	if (recv)
+		p->owned.rels[p->owned.nrels++] = recv;
+	if (rc)
+		return rc;
+	/* an error this segment's own kernels raised (fetched with the completion: no extra round trip) is
+	 * the one to report here; the peers see CBGPU_ERR_PEER */
+	{
+		char		peermsg[512];
+		int			st;
+
+		snprintf(peermsg, sizeof(peermsg), "%s", rc2 ? cbgpu_last_error(es->es_ctx) : "");
+		st = cbgpu_check_status(es->es_ctx);
+		if (st)
+		{
+			es->es_errcode = 0;
+			return es_fail(es, st, "%s", cbgpu_last_error(es->es_ctx));
+		}
+		if (rc2)
+			return es->es_errcode ? es->es_errcode : es_fail(es, rc2, "%s", peermsg);
+	}
+	ps->instrument.kernels += cbgpu_kernel_launches(es->es_ctx) - before;
+	ps->instrument.rows_in += s->rows_in;
+	if (cbgpu_last_kernel_ms(es->es_ctx) > 0)
+		ps->instrument.device_ms += cbgpu_last_kernel_ms(es->es_ctx);
+	if (outcome == CBGPU_DX_DELIVERED)
+	{
+		/* RecvTupleFrom for the whole stream, done */
+		memset(&pl->sink, 0, sizeof(pl->sink));
+		p->recv = recv;
+		p->recv_ready = 1;
+		p->xstage = 2;
+		*send = rel;
+		*delivered = 1;
+		return CBGPU_OK;
+	}
+	/* CBGPU_DX_RETRY: a destination's window was full somewhere (skew, or a Motion larger than the
+	 * windows): every segment redoes it staged, with exactly sized buffers */
+	pl->sink.part_cols = NULL;
+	pl->sink.part_counts = NULL;
+	pl->sink.part_nulls = NULL;
+	pl->sink.part_nullmask = 0;
+	return CBGPU_OK;
+}
+
+/* staged Motion: partition into a local send buffer, then the interconnect's exchange.  First an
+ * optimistic layout (every destination could receive every row: reserve nrows per destination only
+ * when small, otherwise the even share plus a skew allowance); if a destination turns out fuller -
+ * the reference never fails on skew, it sends tuple by tuple (cdbmotion.c:425) - the counts of that
+ * pass size a second, exact one */
+static int
+motion_send_staged(CbPlanState *ps, CbStream *s, const SinkLayout *lay, void *counter, int64_t *counts, int64_t *offsets,
+				   cbgpu_rel **send)
+{
+	CbEState   *es = ps->state;
+	CbMotion   *m = (CbMotion *) ps->plan;
+	NodePriv   *p = np(ps);
+	CbPipeline *pl = &s->pipe;
+	const int	nsegs = es->es_numsegments;
+	int64_t		base[64],
+				cap[64];
+	int64_t		each = pl->nrows;
+	int64_t		total = 0;
+	int			over = 0;
+	void	   *flagword = (char *) counter + sizeof(int64_t) * (size_t) nsegs;
+	cbgpu_rel  *rel;
+
+	if (pl->nrows > (1 << 20))
+	{
+		each = pl->nrows / nsegs + pl->nrows / (4 * nsegs) + 65536;
+		if (each > pl->nrows)
+			each = pl->nrows;
+	}
+	for (int d = 0; d < nsegs; d++)
+	{
+		base[d] = (int64_t) d * each;
+		cap[d] = each;
+	}
+	TRY(rel_create_for_sink(es, &p->owned, lay, each * nsegs, &rel));
+	TRY(partition_pass(ps, s, rel, counter, flagword, base, cap, nsegs, counts));
+	for (int d = 0; d < nsegs; d++)
+	{
+		over |= counts[d] > cap[d];
+		total += counts[d];
+	}
+	if (over)
+	{
+		int64_t		again[64];
+
+		for (int d = 0; d < nsegs; d++)
+		{
+			base[d] = d == 0 ? 0 : base[d - 1] + counts[d - 1];
+			cap[d] = counts[d];
+		}
+		/* the first buffer goes back before the exact one is taken */
+		for (int i = 0; i < p->owned.nrels; i++)
+			if (p->owned.rels[i] == rel)
+				p->owned.rels[i] = p->owned.rels[--p->owned.nrels];
+		cbgpu_rel_free(rel);
+		TRY(rel_create_for_sink(es, &p->owned, lay, total, &rel));
+		TRY(partition_pass(ps, s, rel, counter, flagword, base, cap, nsegs, again));
+		for (int d = 0; d < nsegs; d++)
+			if (again[d] != counts[d])
+				return es_fail(es, CBGPU_ERR_INVALID, "Motion %d: the sender slice routed %lld rows to segment %d on its second pass, %lld on its first",
+							   m->motionID, (long long) again[d], d, (long long) counts[d]);
+		ps->instrument.motion_repartitions += 1;
+	}
+	for (int d = 0; d < nsegs; d++)
+		offsets[d] = base[d];
+	pl->sink.seg_base = NULL;	/* they pointed into this frame */
+	pl->sink.seg_cap = NULL;
+	*send = rel;
+	return CBGPU_OK;
+}
+
 /* execMotionSender (nodeMotion.c:203): run the child, route every row.  Leaves either the delivered rows in
  * np(ps)->recv (direct Motion: recv_ready set) or this segment's rows grouped by destination in *send
  * (destination d: offsets[d], counts[d]).  np(ps)->xstage tells open_motion how far the exchange got, for
@@ -2365,6 +2567,14 @@ motion_send_side(CbPlanState *ps, cbgpu_rel **send, int64_t *counts, int64_t *of
 	NodePriv   *p = np(ps);
 	CbStream   *s;
 	int			nsegs = es->es_numsegments;
+	CbPipeline *pl;
+	int			saved_nops;
+	int			hashpe[CBP_MAX_KEYS];
+	int			outer[MAX_OUT];
+	VarCtx		vc;
+	SinkLayout	lay;
+	void	   *counter;
+	int			delivered = 0;
 
 	TRY(node_open(ps->lefttree, &s));
 	if (m->motionType != CB_MOTIONTYPE_HASH)
@@ -2375,290 +2585,52 @@ motion_send_side(CbPlanState *ps, cbgpu_rel **send, int64_t *counts, int64_t *of
 		return CBGPU_OK;
 	}
 	/* hash motion: PARTITION sink = evalHashKey (nodeMotion.c:1088) + per-destination buffers */
+	pl = &s->pipe;
+	saved_nops = pl->nops;
+	if (m->nhashExprs < 1 || m->nhashExprs > CBP_MAX_KEYS)
+		return es_fail(es, CBGPU_ERR_UNSUPPORTED, "hash Motion with %d keys is beyond the GPU path's limit", m->nhashExprs);
+	memcpy(outer, s->out, sizeof(int) * (size_t) s->nout);
+	memset(&vc, 0, sizeof(vc));
+	vc.es = es;
+	vc.s = s;
+	vc.outer = outer;
+	vc.nouter = s->nout;
+	memset(&pl->sink, 0, sizeof(pl->sink));
+	for (int k = 0; k < m->nhashExprs; k++)
 	{
-		int32_t		types[CBP_MAX_OUT],
-					dscales[CBP_MAX_OUT];
-		int			ncols = 0,
-					nullable[CBP_MAX_OUT];
-		CbPipeline *pl = &s->pipe;
-		int			saved_nops = pl->nops;
-		int			hashpe[CBP_MAX_KEYS];
-		int			outer[MAX_OUT];
-		VarCtx		vc;
-		void	   *counter;
-		cbgpu_rel  *rel;
-		uint64_t	nullmask = 0;
+		PExpr	   *kx;
 
-		if (m->nhashExprs < 1 || m->nhashExprs > CBP_MAX_KEYS)
-			return es_fail(es, CBGPU_ERR_UNSUPPORTED, "hash Motion with %d keys is beyond the GPU path's limit", m->nhashExprs);
-		memcpy(outer, s->out, sizeof(int) * (size_t) s->nout);
-		memset(&vc, 0, sizeof(vc));
-		vc.es = es;
-		vc.s = s;
-		vc.outer = outer;
-		vc.nouter = s->nout;
-		/* the hash key values go first on the stack (and into the leading output columns),
-		 * then every output column */
-		memset(&pl->sink, 0, sizeof(pl->sink));
-		for (int k = 0; k < m->nhashExprs; k++)
+		TRY(translate(&vc, m->hashExprs[k], &hashpe[k]));
+		kx = &s->pe[hashpe[k]];
+		if (kx->kind == PE_STATE || kx->type == CB_NUMERIC)
+			return es_fail(es, CBGPU_ERR_UNSUPPORTED, "Motion hash key type is not supported on the GPU path");
+		pl->sink.hashtype[k] = kx->type;
+		if (kx->type == CB_DICT8 || kx->type == CB_DICT32)
 		{
-			PExpr	   *kx;
-
-			TRY(translate(&vc, m->hashExprs[k], &hashpe[k]));
-			kx = &s->pe[hashpe[k]];
-			if (kx->kind == PE_STATE || kx->type == CB_NUMERIC)
-				return es_fail(es, CBGPU_ERR_UNSUPPORTED, "Motion hash key type is not supported on the GPU path");
-			TRY(emit_expr(es, s, hashpe[k]));
-			types[ncols] = kx->type;
-			dscales[ncols] = kx->dscale;
-			nullable[ncols] = kx->maybe_null;
-			pl->sink.hashtype[k] = kx->type;
-			if (kx->type == CB_DICT8 || kx->type == CB_DICT32)
-			{
-				if (kx->kind != PE_COL || !pl->cols[kx->col].dict_hash)
-					return es_fail(es, CBGPU_ERR_INVALID, "dictionary Motion key without per-code hashes");
-				pl->sink.hash_dict_hash[k] = pl->cols[kx->col].dict_hash;
-			}
-			ncols++;
-		}
-		for (int i = 0; i < s->nout; i++)
-		{
-			PExpr	   *x = &s->pe[s->out[i]];
-
-			p->send_pe[i] = *x;
-			if (x->kind == PE_STATE)
-			{
-				if (ncols + 3 > CBP_MAX_OUT)
-					return es_fail(es, CBGPU_ERR_UNSUPPORTED, "too many Motion columns");
-				for (int k = 0; k < 3; k++)
-				{
-					types[ncols] = CB_INT8;
-					dscales[ncols] = 0;
-					nullable[ncols] = 0;
-					ncols++;
-				}
-				TRY(emit_expr(es, s, x->cn));
-				TRY(emit_expr(es, s, x->clo));
-				TRY(emit_expr(es, s, x->chi));
-			}
-			else
-			{
-				if (ncols + 1 > CBP_MAX_OUT)
-					return es_fail(es, CBGPU_ERR_UNSUPPORTED, "too many Motion columns");
-				types[ncols] = x->type;
-				dscales[ncols] = x->dscale;
-				nullable[ncols] = x->maybe_null;
-				ncols++;
-				TRY(emit_expr(es, s, s->out[i]));
-			}
-		}
-		p->send_nout = s->nout;
-		TRY(emit_op(es, s, CBP_END, 0, 0));
-		GPU(es, cbgpu_dev_alloc(es->es_ctx, sizeof(int64_t) * (size_t) (nsegs + 1), &counter));
-		p->owned.devs[p->owned.ndevs++] = counter;
-		pl->sink.kind = CBP_SINK_PARTITION;
-		pl->sink.nout = ncols;
-		pl->sink.out_count = (int64_t *) counter;
-		pl->sink.nhash = m->nhashExprs;
-		pl->sink.nsegs = m->numHashSegments > 0 ? m->numHashSegments : nsegs;
-		pl->force_generic = es->es_force_generic;
-		if (pl->sink.nsegs != nsegs)
-			return es_fail(es, CBGPU_ERR_UNSUPPORTED, "Motion to %d hash segments on a %d-segment cluster", pl->sink.nsegs, nsegs);
-		for (int c = 0; c < ncols; c++)
-			if (nullable[c])
-				nullmask |= 1ull << c;
-
-		/* direct Motion (interconnects with peer memory): the PARTITION sink stores every row straight into
-		 * its destination segment's receive window - no send buffer, no separate exchange, no collective */
-		{
-			CbInterconnect *ic = es->es_cluster ? NULL : es->es_interconnect;
-			cbgpu_direct_dest dest;
-
-			if (ic && ic->direct_begin && ic->direct_begin(ic, es, m->motionID, ncols, types, dscales, &dest) == CBGPU_OK)
-			{
-				cbgpu_rel  *recv = NULL;
-				int32_t		outcome = CBGPU_DX_DELIVERED;
-				int			rc,
-							rc2;
-				int64_t		before = cbgpu_kernel_launches(es->es_ctx);
-
-				/* from here to direct_end nothing may return early: the peers wait for this segment's signal */
-				rc = cbgpu_rel_create(es->es_ctx, 0, ncols, types, dscales, &rel);
-				if (rc == CBGPU_OK)
-				{
-					p->owned.rels[p->owned.nrels++] = rel;
-					pl->sink.out = rel;
-					pl->sink.seg_capacity = dest.capacity;
-					pl->sink.part_cols = dest.cols;
-					pl->sink.part_counts = dest.counts;
-					pl->sink.part_nulls = dest.nulls;
-					pl->sink.part_nullmask = nullmask;
-					pl->sink.part_flags = dest.flags;
-					rc = run_pipeline(es, pl);
-				}
-				if (rc && es->es_errcode == 0)
-					es_fail(es, rc, "%s", cbgpu_last_error(es->es_ctx));
-				rc2 = ic->direct_end(ic, es, m->motionID, rc ? CBGPU_DX_ERROR : 0, nullmask, (const int64_t *) counter, counts, &recv, &outcome);
-				p->xstage = 1;
-				if (recv)
-					p->owned.rels[p->owned.nrels++] = recv;
-				if (rc)
-					return rc;
-				/* an error this segment's own kernels raised (fetched with the completion: no extra round trip) is
-				 * the one to report here; the peers see CBGPU_ERR_PEER */
-				{
-					char		peermsg[512];
-					int			st;
-
-					snprintf(peermsg, sizeof(peermsg), "%s", rc2 ? cbgpu_last_error(es->es_ctx) : "");
-					st = cbgpu_check_status(es->es_ctx);
-					if (st)
-					{
-						es->es_errcode = 0;
-						return es_fail(es, st, "%s", cbgpu_last_error(es->es_ctx));
-					}
-					if (rc2)
-						return es->es_errcode ? es->es_errcode : es_fail(es, rc2, "%s", peermsg);
-				}
-				ps->instrument.kernels += cbgpu_kernel_launches(es->es_ctx) - before;
-				ps->instrument.rows_in += s->rows_in;
-				if (cbgpu_last_kernel_ms(es->es_ctx) > 0)
-					ps->instrument.device_ms += cbgpu_last_kernel_ms(es->es_ctx);
-				if (outcome == CBGPU_DX_DELIVERED)
-				{
-					/* RecvTupleFrom for the whole stream, done */
-					int			c = m->nhashExprs;
-
-					for (int k = 0; k < m->nhashExprs; k++)
-					{
-						PExpr	   *kx = &s->pe[hashpe[k]];
-
-						if (kx->kind == PE_COL && (kx->type == CB_DICT8 || kx->type == CB_DICT32) && pl->cols[kx->col].dict_hash)
-							GPU(es, cbgpu_rel_share_dict_hash(recv, k, s->col_rel[kx->col], s->col_idx[kx->col]));
-					}
-					for (int i = 0; i < s->nout; i++)
-					{
-						PExpr	   *x = &s->pe[s->out[i]];
-
-						if (x->kind == PE_STATE)
-						{
-							c += 3;
-							continue;
-						}
-						if (x->kind == PE_COL && (x->type == CB_DICT8 || x->type == CB_DICT32) && pl->cols[x->col].dict_hash)
-							GPU(es, cbgpu_rel_share_dict_hash(recv, c, s->col_rel[x->col], s->col_idx[x->col]));
-						c++;
-					}
-					pl->nops = saved_nops;
-					memset(&pl->sink, 0, sizeof(pl->sink));
-					p->recv = recv;
-					p->recv_ready = 1;
-					p->xstage = 2;
-					*send = rel;
-					return CBGPU_OK;
-				}
-				/* CBGPU_DX_RETRY: a destination's window was full somewhere (skew, or a Motion larger than the
-				 * windows): every segment redoes it staged, with exactly sized buffers */
-				pl->sink.part_cols = NULL;
-				pl->sink.part_counts = NULL;
-				pl->sink.part_nulls = NULL;
-				pl->sink.part_nullmask = 0;
-			}
-		}
-
-		/* staged Motion: partition into a local send buffer, then the interconnect's exchange.  First an
-		 * optimistic layout (every destination could receive every row: reserve nrows per destination only
-		 * when small, otherwise the even share plus a skew allowance); if a destination turns out fuller -
-		 * the reference never fails on skew, it sends tuple by tuple (cdbmotion.c:425) - the counts of that
-		 * pass size a second, exact one */
-		{
-			int64_t		base[64],
-						cap[64];
-			int64_t		each = pl->nrows;
-			int64_t		total = 0;
-			int			over = 0;
-			void	   *flagword = (char *) counter + sizeof(int64_t) * (size_t) nsegs;
-
-			if (pl->nrows > (1 << 20))
-			{
-				each = pl->nrows / nsegs + pl->nrows / (4 * nsegs) + 65536;
-				if (each > pl->nrows)
-					each = pl->nrows;
-			}
-			for (int d = 0; d < nsegs; d++)
-			{
-				base[d] = (int64_t) d * each;
-				cap[d] = each;
-			}
-			GPU(es, cbgpu_rel_create(es->es_ctx, each * nsegs, ncols, types, dscales, &rel));
-			p->owned.rels[p->owned.nrels++] = rel;
-			for (int c = 0; c < ncols; c++)
-				if (nullable[c])
-					GPU(es, cbgpu_rel_add_nullmap(rel, c));
-			TRY(partition_pass(ps, s, rel, counter, flagword, base, cap, nsegs, counts));
-			for (int d = 0; d < nsegs; d++)
-			{
-				over |= counts[d] > cap[d];
-				total += counts[d];
-			}
-			if (over)
-			{
-				int64_t		again[64];
-
-				for (int d = 0; d < nsegs; d++)
-				{
-					base[d] = d == 0 ? 0 : base[d - 1] + counts[d - 1];
-					cap[d] = counts[d];
-				}
-				/* the first buffer goes back before the exact one is taken */
-				for (int i = 0; i < p->owned.nrels; i++)
-					if (p->owned.rels[i] == rel)
-						p->owned.rels[i] = p->owned.rels[--p->owned.nrels];
-				cbgpu_rel_free(rel);
-				GPU(es, cbgpu_rel_create(es->es_ctx, total, ncols, types, dscales, &rel));
-				p->owned.rels[p->owned.nrels++] = rel;
-				for (int c = 0; c < ncols; c++)
-					if (nullable[c])
-						GPU(es, cbgpu_rel_add_nullmap(rel, c));
-				TRY(partition_pass(ps, s, rel, counter, flagword, base, cap, nsegs, again));
-				for (int d = 0; d < nsegs; d++)
-					if (again[d] != counts[d])
-						return es_fail(es, CBGPU_ERR_INVALID, "Motion %d: the sender slice routed %lld rows to segment %d on its second pass, %lld on its first",
-									   m->motionID, (long long) again[d], d, (long long) counts[d]);
-				ps->instrument.motion_repartitions += 1;
-			}
-			for (int d = 0; d < nsegs; d++)
-				offsets[d] = base[d];
-			{
-				int			c = m->nhashExprs;
-
-				for (int i = 0; i < s->nout; i++)
-				{
-					PExpr	   *x = &s->pe[s->out[i]];
-
-					if (x->kind == PE_STATE)
-					{
-						c += 3;
-						continue;
-					}
-					if (x->kind == PE_COL && (x->type == CB_DICT8 || x->type == CB_DICT32) && pl->cols[x->col].dict_hash)
-						GPU(es, cbgpu_rel_share_dict_hash(rel, c, s->col_rel[x->col], s->col_idx[x->col]));
-					c++;
-				}
-				for (int k = 0; k < m->nhashExprs; k++)
-				{
-					PExpr	   *kx = &s->pe[hashpe[k]];
-
-					if (kx->kind == PE_COL && (kx->type == CB_DICT8 || kx->type == CB_DICT32) && pl->cols[kx->col].dict_hash)
-						GPU(es, cbgpu_rel_share_dict_hash(rel, k, s->col_rel[kx->col], s->col_idx[kx->col]));
-				}
-			}
-			pl->nops = saved_nops;
-			pl->sink.seg_base = NULL;	/* they pointed into this frame */
-			pl->sink.seg_cap = NULL;
-			*send = rel;
+			if (kx->kind != PE_COL || !pl->cols[kx->col].dict_hash)
+				return es_fail(es, CBGPU_ERR_INVALID, "dictionary Motion key without per-code hashes");
+			pl->sink.hash_dict_hash[k] = pl->cols[kx->col].dict_hash;
 		}
 	}
+	/* the hash key values go first on the stack (and into the leading output columns),
+	 * then every output column */
+	TRY(emit_sink_columns(es, s, hashpe, m->nhashExprs, &lay, p->send_pe));
+	p->send_nout = s->nout;
+	GPU(es, cbgpu_dev_alloc(es->es_ctx, sizeof(int64_t) * (size_t) (nsegs + 1), &counter));
+	p->owned.devs[p->owned.ndevs++] = counter;
+	pl->sink.kind = CBP_SINK_PARTITION;
+	pl->sink.nout = lay.ncols;
+	pl->sink.out_count = (int64_t *) counter;
+	pl->sink.nhash = m->nhashExprs;
+	pl->sink.nsegs = m->numHashSegments > 0 ? m->numHashSegments : nsegs;
+	pl->force_generic = es->es_force_generic;
+	if (pl->sink.nsegs != nsegs)
+		return es_fail(es, CBGPU_ERR_UNSUPPORTED, "Motion to %d hash segments on a %d-segment cluster", pl->sink.nsegs, nsegs);
+	TRY(motion_send_direct(ps, s, &lay, counter, counts, send, &delivered));
+	if (!delivered)
+		TRY(motion_send_staged(ps, s, &lay, counter, counts, offsets, send));
+	TRY(rel_share_dicts(es, delivered ? p->recv : *send, s, hashpe, m->nhashExprs, p->send_pe, p->send_nout));
+	pl->nops = saved_nops;
 	return CBGPU_OK;
 }
 
@@ -2671,34 +2643,8 @@ motion_recv_stream(CbPlanState *ps, cbgpu_rel *recv, CbStream **out)
 	NodePriv   *p = np(ps);
 	CbStream   *s = stream_new(p);
 	int			lead = m->motionType == CB_MOTIONTYPE_HASH ? m->nhashExprs : 0;
-	int			c = lead;
 
-	s->pipe.nrows = cbgpu_rel_nrows(recv);
-	s->rows_in = s->pipe.nrows;
-	s->nsrc = 1;
-	s->nout = p->send_nout;
-	for (int i = 0; i < p->send_nout; i++)
-	{
-		if (p->send_pe[i].kind == PE_STATE)
-		{
-			PExpr		e = p->send_pe[i];
-
-			e.cn = pe_col(s, recv, c, 0, 0);
-			e.clo = pe_col(s, recv, c + 1, 0, 0);
-			e.chi = pe_col(s, recv, c + 2, 0, 0);
-			s->out[i] = (e.cn < 0 || e.clo < 0 || e.chi < 0) ? -1 : pe_add(s, &e);
-			c += 3;
-		}
-		else
-		{
-			s->out[i] = pe_col(s, recv, c, 0, 0);
-			if (s->out[i] >= 0)
-				s->pe[s->out[i]].dscale = p->send_pe[i].dscale;
-			c++;
-		}
-		if (s->out[i] < 0)
-			return es_fail(es, CBGPU_ERR_UNSUPPORTED, "too many columns in one pipeline");
-	}
+	TRY(stream_over_rel(es, s, recv, p->send_pe, p->send_nout, lead));
 	if (m->nsortkeys > 0 && s->pipe.nrows > 1)
 	{
 		/* merge receive (execMotionSortedReceiver, nodeMotion.c:433): the senders' sorted streams lie one after another
@@ -2943,10 +2889,13 @@ rel_to_result(CbEState *es, cbgpu_rel *rel, const PExpr *shape, int nshape, cons
 	}
 	if (rc == CBGPU_OK)
 	{
-		int			c = 0;
+		int			colstart[MAX_OUT];
 
+		shape_columns(shape, nshape, 0, colstart);
 		for (int i = 0; i < nshape; i++)
 		{
+			const int	c = colstart[i];
+
 			if (shape[i].kind == PE_STATE)
 			{
 				for (int64_t r = 0; r < nrows; r++)
@@ -2971,7 +2920,6 @@ rel_to_result(CbEState *es, cbgpu_rel *rel, const PExpr *shape, int nshape, cons
 				}
 				if (nrows == 0)
 					rs->types[i] = shape[i].restype;
-				c += 3;
 			}
 			else
 			{
@@ -2994,7 +2942,6 @@ rel_to_result(CbEState *es, cbgpu_rel *rel, const PExpr *shape, int nshape, cons
 					else
 						rs->vals[o] = colv[c][r];
 				}
-				c++;
 			}
 		}
 	}
@@ -3022,14 +2969,9 @@ sort_key_columns(CbEState *es, const PExpr *shape, int nshape, int lead, const C
 				 int32_t *desc, int32_t *uns, int *nk_out)
 {
 	int			colstart[MAX_OUT];
-	int			c = lead;
 	int			nk = 0;
 
-	for (int i = 0; i < nshape; i++)
-	{
-		colstart[i] = c;
-		c += shape[i].kind == PE_STATE ? 3 : 1;
-	}
+	shape_columns(shape, nshape, lead, colstart);
 	for (int k = 0; k < nkeys; k++)
 	{
 		int			att = keys[k].attno;
@@ -3104,33 +3046,16 @@ limitsort_run(CbPlanState *ps, cbgpu_rel **out_rel, PExpr *out_shape, int *out_n
 		ps->instrument.kernels += cbgpu_kernel_launches(es->es_ctx) - before;
 	}
 	/* the chosen rows, in order, as a small relation of their own */
+	TRY(rel_create_like(es, &p->owned, rel, nout, out_rel));
+	if (nout > 0)
 	{
-		int32_t		types[CBP_MAX_OUT],
-					dscales[CBP_MAX_OUT];
-		int			ncols = cbgpu_rel_ncols(rel);
-		cbgpu_rel  *small;
+		/* one gather kernel for all rows and columns (row-by-row copies were 60 tiny memcpys for Q3's ten rows) */
+		void	   *didx;
 
-		for (int c = 0; c < ncols; c++)
-		{
-			types[c] = cbgpu_rel_col_type(rel, c);
-			dscales[c] = cbgpu_rel_col_dscale(rel, c);
-		}
-		GPU(es, cbgpu_rel_create(es->es_ctx, nout, ncols, types, dscales, &small));
-		p->owned.rels[p->owned.nrels++] = small;
-		if (nout > 0)
-		{
-			/* one gather kernel for all rows and columns (row-by-row copies were 60 tiny memcpys for Q3's ten rows) */
-			void	   *didx;
-
-			GPU(es, cbgpu_dev_alloc(es->es_ctx, sizeof(uint32_t) * (size_t) nout, &didx));
-			p->owned.devs[p->owned.ndevs++] = didx;
-			GPU(es, cbgpu_dev_write(es->es_ctx, didx, sizeof(uint32_t) * (size_t) nout, idx));
-			GPU(es, cbgpu_rel_take_rows(small, rel, (const uint32_t *) didx, nout));
-		}
-		for (int c = 0; c < ncols; c++)
-			if (cbgpu_rel_dict_hash_dev(rel, c))
-				GPU(es, cbgpu_rel_share_dict_hash(small, c, rel, c));
-		*out_rel = small;
+		GPU(es, cbgpu_dev_alloc(es->es_ctx, sizeof(uint32_t) * (size_t) nout, &didx));
+		p->owned.devs[p->owned.ndevs++] = didx;
+		GPU(es, cbgpu_dev_write(es->es_ctx, didx, sizeof(uint32_t) * (size_t) nout, idx));
+		GPU(es, cbgpu_rel_take_rows(*out_rel, rel, (const uint32_t *) didx, nout));
 	}
 	memcpy(out_shape, shape, sizeof(PExpr) * (size_t) nshape);
 	*out_nshape = nshape;
@@ -3158,7 +3083,7 @@ open_limitsort(CbPlanState *ps, CbStream **out)
 
 	TRY(limitsort_run(ps, &small, shape, &nshape));
 	s = stream_new(np(ps));
-	TRY(stream_over_rel(ps->state, s, small, shape, nshape));
+	TRY(stream_over_rel(ps->state, s, small, shape, nshape, 0));
 	*out = s;
 	return CBGPU_OK;
 }
@@ -3186,49 +3111,17 @@ node_result(CbPlanState *ps)
 		const uint32_t *sel = NULL;
 
 		TRY(node_open(ps, &s));
-		if (stream_is_plain(s, &rel, &sel))
+		/* already a relation with exactly these columns?  (Motion receive buffers, agg relations) */
+		if (stream_is_plain(s, &rel, &sel) && stream_is_rel_layout(s, rel, shape))
 		{
-			/* already a relation with exactly these columns?  (Motion receive buffers, agg relations) */
-			int			exact = 1,
-						c = 0;
+			cbgpu_rel  *ordered;
 
-			for (int i = 0; i < s->nout && exact; i++)
-			{
-				PExpr	   *x = &s->pe[s->out[i]];
-
-				shape[i] = *x;
-				if (x->kind == PE_STATE)
-				{
-					if (s->pe[x->cn].kind != PE_COL || s->col_idx[s->pe[x->cn].col] != c)
-						exact = 0;
-					c += 3;
-				}
-				else
-				{
-					if (x->kind != PE_COL || s->col_idx[x->col] != c)
-						exact = 0;
-					c++;
-				}
-			}
-			if (exact && c == cbgpu_rel_ncols(rel) && !sel)
+			if (!sel)
 				return rel_to_result(es, rel, shape, s->nout, NULL, 0, &p->rs);
-			if (exact && c == cbgpu_rel_ncols(rel))
-			{
-				/* the rows in the stream's order (a MATERIALIZE sink appends in whatever order its warps finish) */
-				int32_t		types[CBP_MAX_OUT],
-							dscales[CBP_MAX_OUT];
-				cbgpu_rel  *ordered;
-
-				for (int k = 0; k < c; k++)
-				{
-					types[k] = cbgpu_rel_col_type(rel, k);
-					dscales[k] = cbgpu_rel_col_dscale(rel, k);
-				}
-				GPU(es, cbgpu_rel_create(es->es_ctx, s->pipe.nrows, c, types, dscales, &ordered));
-				p->owned.rels[p->owned.nrels++] = ordered;
-				GPU(es, cbgpu_rel_take_rows(ordered, rel, sel, s->pipe.nrows));
-				return rel_to_result(es, ordered, shape, s->nout, NULL, 0, &p->rs);
-			}
+			/* the rows in the stream's order (a MATERIALIZE sink appends in whatever order its warps finish) */
+			TRY(rel_create_like(es, &p->owned, rel, s->pipe.nrows, &ordered));
+			GPU(es, cbgpu_rel_take_rows(ordered, rel, sel, s->pipe.nrows));
+			return rel_to_result(es, ordered, shape, s->nout, NULL, 0, &p->rs);
 		}
 		TRY(stream_materialize(es, ps, s, &p->owned, &rel, shape, &nshape));
 		return rel_to_result(es, rel, shape, nshape, NULL, 0, &p->rs);
@@ -3756,9 +3649,6 @@ cluster_run_motion(CbPlanState *me)
 		int64_t		total = 0;
 		cbgpu_rel  *recv = NULL;
 		cbgpu_rel  *shape_src = NULL;
-		int32_t		types[CBP_MAX_OUT],
-					dscales[CBP_MAX_OUT];
-		int			ncols;
 		int64_t		off = 0;
 		NodePriv   *dp = np(mps[d]);
 
@@ -3788,22 +3678,9 @@ cluster_run_motion(CbPlanState *me)
 			rc = es_fail(me->state, CBGPU_ERR_INVALID, "Motion %d: no sender ran", m->motionID);
 			break;
 		}
-		ncols = cbgpu_rel_ncols(shape_src);
-		for (int k = 0; k < ncols; k++)
-		{
-			types[k] = cbgpu_rel_col_type(shape_src, k);
-			dscales[k] = cbgpu_rel_col_dscale(shape_src, k);
-		}
-		rc = cbgpu_rel_create(c->ctx, total, ncols, types, dscales, &recv);
+		rc = rel_create_like(me->state, &dp->owned, shape_src, total, &recv);
 		if (rc)
-		{
-			es_fail(me->state, rc, "%s", cbgpu_last_error(c->ctx));
 			break;
-		}
-		dp->owned.rels[dp->owned.nrels++] = recv;
-		for (int k = 0; k < ncols; k++)
-			if (cbgpu_rel_dict_hash_dev(shape_src, k))
-				cbgpu_rel_share_dict_hash(recv, k, shape_src, k);
 		for (int s = 0; s < nsegs && rc == CBGPU_OK; s++)
 		{
 			int64_t		n = 0,
