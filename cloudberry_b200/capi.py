@@ -370,6 +370,11 @@ def gpu():
             "cbgpu_pairs_free": (None, [vp]),
             "cbgpu_merge_sorted_runs": (C.c_int, [vp, vp, C.POINTER(i32), C.POINTER(i32), C.POINTER(i32), i32, i32, C.POINTER(vp),
                                                   C.POINTER(i32)]),
+            "cbgpu_topn": (C.c_int, [vp, vp, C.POINTER(i32), C.POINTER(i32), C.POINTER(i32), i32, i64, C.POINTER(C.c_uint32),
+                                     C.POINTER(i64)]),
+            "cbgpu_rel_take_rows": (C.c_int, [vp, vp, vp, i64]),
+            "cbgpu_dev_alloc": (C.c_int, [vp, C.c_size_t, C.POINTER(vp)]),
+            "cbgpu_dev_write": (C.c_int, [vp, vp, C.c_size_t, vp]),
             "cbgpu_dev_free": (None, [vp, vp]),
             "cbgpu_read_u32": (C.c_int, [vp, vp, i64, vp]),
             "cbgpu_motion_unique_id": (C.c_int, [vp]),

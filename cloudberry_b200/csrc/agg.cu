@@ -621,7 +621,7 @@ k_topn_min(TopnParams p, int keyi, unsigned long long *bmin, unsigned long long 
 	__syncthreads();
 	if (threadIdx.x == 0)
 	{
-		for (int w = 1; w < 8; w++)
+		for (int w = 1; w < (int) (blockDim.x >> 5); w++)
 		{
 			lo = smin[w] < lo ? smin[w] : lo;
 			hi = smax[w] > hi ? smax[w] : hi;
@@ -959,16 +959,23 @@ cbgpu_topn(cbgpu_ctx *ctx, cbgpu_rel *rel, const int32_t *keycols, const int32_t
 		}
 		else
 		{
-			int			nblocks = (int) ((rel->nrows + 63) / 64);	/* > TOPN_CAND rows: at least TOPN_MAXK blocks */
+			/* every block of k_topn_min must see a row: an empty block's minimum is ~0, and when fewer than k blocks hold
+			 * rows the k-th smallest minimum admits every row.  At most one block per 64 rows, each of 256 threads halved
+			 * down to 64 until the grid's last block starts inside the rows: > TOPN_CAND rows give > TOPN_MAXK blocks,
+			 * all with rows */
+			int			nblocks = (int) ((rel->nrows + 63) / 64);
+			int			tpb = 256;
 
 			if (nblocks > TOPN_BLOCKS)
 				nblocks = TOPN_BLOCKS;
+			while (tpb > 64 && (int64_t) (nblocks - 1) * tpb >= rel->nrows)
+				tpb >>= 1;
 			CB_CUDA(ctx, cudaMallocAsync(&scratch, (2 * TOPN_BLOCKS + 3) * sizeof(unsigned long long), ctx->stream));
 			CB_CUDA(ctx, cudaMallocAsync(&cand, TOPN_CAND * sizeof(uint32_t), ctx->stream));
 			CB_CUDA(ctx, cudaMallocAsync(&ncand, sizeof(int), ctx->stream));
 			for (int keyi = 0; keyi < nkeys && !done; keyi++)
 			{
-				k_topn_min<<<nblocks, 256, 0, ctx->stream>>>(p, keyi, scratch, scratch + TOPN_BLOCKS);
+				k_topn_min<<<nblocks, tpb, 0, ctx->stream>>>(p, keyi, scratch, scratch + TOPN_BLOCKS);
 				CB_LAUNCHED(ctx, "k_topn_min");
 				k_topn_kth<<<1, TOPN_BLOCKS, 0, ctx->stream>>>(scratch, scratch + TOPN_BLOCKS, nblocks, p.k, scratch + 2 * TOPN_BLOCKS);
 				CB_LAUNCHED(ctx, "k_topn_kth");
@@ -998,11 +1005,12 @@ cbgpu_topn(cbgpu_ctx *ctx, cbgpu_rel *rel, const int32_t *keycols, const int32_t
 		CB_CUDA(ctx, cudaFreeAsync(cand1, ctx->stream));
 		cand1 = NULL;
 	}
-	/* tournament: every pass gives each thread ~64 candidates and keeps its best k, until one thread
-	 * holds the answer; passes shrink the candidate list by ~64 / k each */
+	/* tournament: every pass gives each thread up to per_thread candidates and keeps its best k, until one
+	 * thread holds the answer.  per_thread >= 4k, so a pass leaves at most half its input (k per thread,
+	 * padded); a pass that does not shrink its input is an error, never an endless loop */
 	{
 		const int	threads = 128;
-		const int64_t per_thread = 64;
+		const int64_t per_thread = limit * 4 > 64 ? limit * 4 : 64;
 		const uint32_t *in = NULL;
 		int64_t		nin = rel->nrows;
 		int			which = 0;
@@ -1033,6 +1041,12 @@ cbgpu_topn(cbgpu_ctx *ctx, cbgpu_rel *rel, const int32_t *keycols, const int32_t
 				if (outbuf != cand1)
 					CB_CUDA(ctx, cudaMemcpyAsync(cand1, outbuf, limit * sizeof(uint32_t), cudaMemcpyDeviceToDevice, ctx->stream));
 				break;
+			}
+			if (n1 >= nin)
+			{
+				cudaFreeAsync(cand1, ctx->stream);
+				cudaFreeAsync(cand2, ctx->stream);
+				return cb_fail(ctx, CBGPU_ERR_INVALID, "device top-N: a tournament pass did not shrink its input%s (%lld candidates)", "", nin);
 			}
 			in = outbuf;
 			nin = n1;
