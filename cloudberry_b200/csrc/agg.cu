@@ -80,21 +80,20 @@ extern "C" int
 cbgpu_agg_create(cbgpu_ctx *ctx, int32_t nkeys, int32_t naccs, const int32_t *acc_kinds, int64_t capacity_groups,
 				 cbgpu_aggtable **out)
 {
-	cbgpu_aggtable *t;
 	int64_t		cap;
+	int			rc;
 
+	*out = NULL;
 	if (nkeys < 0 || nkeys > CBP_MAX_KEYS || naccs < 0 || naccs > CBP_MAX_AGGS)
 		return cb_fail(ctx, CBGPU_ERR_UNSUPPORTED, "aggregate with %s%lld keys/accumulators is beyond the GPU path's limits", "", (long long) (nkeys * 100 + naccs));
-	t = (cbgpu_aggtable *) calloc(1, sizeof(cbgpu_aggtable));
+	CbOwned<cbgpu_aggtable> t((cbgpu_aggtable *) calloc(1, sizeof(cbgpu_aggtable)), cbgpu_agg_free);
+
 	if (!t)
 		return CBGPU_ERR_NOMEM;
+	t->ctx = ctx;
 	cap = next_pow2((capacity_groups < 16 ? 16 : capacity_groups) * 2);
 	if (cap > (1ll << 31))
-	{
-		free(t);
 		return cb_fail(ctx, CBGPU_ERR_UNSUPPORTED, "aggregate table of %s%lld slots exceeds the GPU path's limit", "", cap);
-	}
-	t->ctx = ctx;
 	t->capacity = cap;
 	t->d.mask = (uint32_t) (cap - 1);
 	t->d.nkeys = nkeys;
@@ -125,8 +124,9 @@ cbgpu_agg_create(cbgpu_ctx *ctx, int32_t nkeys, int32_t naccs, const int32_t *ac
 		t->d.ngroups = (int32_t *) (base + off[6]);
 	}
 	t->d.full = t->d.ngroups + 1;
-	*out = t;
-	return cbgpu_agg_reset(t);
+	if ((rc = cbgpu_agg_reset(t.get())) == CBGPU_OK)
+		*out = t.release();
+	return rc;
 }
 
 /* device bytes one slot of an aggregate table takes (two slots per group are provisioned: load factor <= 0.5) */
@@ -155,7 +155,8 @@ cbgpu_agg_free(cbgpu_aggtable *t)
 	if (!t)
 		return;
 	cudaSetDevice(t->ctx->device);
-	cudaFreeAsync(t->base, t->ctx->stream);
+	if (t->base)
+		cudaFreeAsync(t->base, t->ctx->stream);
 	free(t->snap);
 	free(t);
 }
@@ -318,6 +319,7 @@ cbgpu_agg_read(cbgpu_aggtable *t, int64_t maxgroups, int64_t *keys, uint32_t *ke
 			   int64_t *sum_hi, int64_t *ngroups)
 {
 	cbgpu_ctx  *ctx = t->ctx;
+	CbCallMem	mem(ctx);
 	int64_t		ng;
 	int			rc = cbgpu_agg_ngroups(t, &ng);
 	AggOut		o;
@@ -349,12 +351,12 @@ cbgpu_agg_read(cbgpu_aggtable *t, int64_t maxgroups, int64_t *keys, uint32_t *ke
 		return CBGPU_OK;
 	}
 	o.maxgroups = ng;
-	CB_CUDA(ctx, cudaMallocAsync(&o.keys, sizeof(int64_t) * ng * nk, ctx->stream));
-	CB_CUDA(ctx, cudaMallocAsync(&o.keynull, sizeof(uint32_t) * ng, ctx->stream));
-	CB_CUDA(ctx, cudaMallocAsync(&o.n, sizeof(int64_t) * ng * na, ctx->stream));
-	CB_CUDA(ctx, cudaMallocAsync(&o.lo, sizeof(int64_t) * ng * na, ctx->stream));
-	CB_CUDA(ctx, cudaMallocAsync(&o.hi, sizeof(int64_t) * ng * na, ctx->stream));
-	CB_CUDA(ctx, cudaMallocAsync(&o.counter, sizeof(int32_t), ctx->stream));
+	CB_CUDA(ctx, mem.alloc(&o.keys, sizeof(int64_t) * ng * nk));
+	CB_CUDA(ctx, mem.alloc(&o.keynull, sizeof(uint32_t) * ng));
+	CB_CUDA(ctx, mem.alloc(&o.n, sizeof(int64_t) * ng * na));
+	CB_CUDA(ctx, mem.alloc(&o.lo, sizeof(int64_t) * ng * na));
+	CB_CUDA(ctx, mem.alloc(&o.hi, sizeof(int64_t) * ng * na));
+	CB_CUDA(ctx, mem.alloc(&o.counter, sizeof(int32_t)));
 	CB_CUDA(ctx, cudaMemsetAsync(o.counter, 0, sizeof(int32_t), ctx->stream));
 	int			blocks = (int) ((t->capacity + 255) / 256);
 
@@ -372,12 +374,6 @@ cbgpu_agg_read(cbgpu_aggtable *t, int64_t maxgroups, int64_t *keys, uint32_t *ke
 		CB_CUDA(ctx, cudaMemcpyAsync(sum_hi, o.hi, sizeof(int64_t) * ng * t->d.naccs, cudaMemcpyDeviceToHost, ctx->stream));
 	}
 	CB_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-	cudaFreeAsync(o.keys, ctx->stream);
-	cudaFreeAsync(o.keynull, ctx->stream);
-	cudaFreeAsync(o.n, ctx->stream);
-	cudaFreeAsync(o.lo, ctx->stream);
-	cudaFreeAsync(o.hi, ctx->stream);
-	cudaFreeAsync(o.counter, ctx->stream);
 	return CBGPU_OK;
 }
 
@@ -448,23 +444,27 @@ extern "C" int
 cbgpu_agg_to_rel(cbgpu_aggtable *t, const int32_t *keytypes, cbgpu_rel **out)
 {
 	cbgpu_ctx  *ctx = t->ctx;
+	CbCallMem	mem(ctx);
 	int64_t		ng;
 	int			rc = cbgpu_agg_ngroups(t, &ng);
 	int32_t		types[CBP_MAX_KEYS + CBP_MAX_AGGS * 3];
 	int			ncols = t->d.nkeys + t->d.naccs * 3;
-	cbgpu_rel  *rel;
+	cbgpu_rel  *created;
 	AggRelOut	o;
 	int			h_flag = 0;
 
+	*out = NULL;
 	if (rc)
 		return rc;
 	for (int k = 0; k < t->d.nkeys; k++)
 		types[k] = keytypes[k];
 	for (int a = 0; a < t->d.naccs * 3; a++)
 		types[t->d.nkeys + a] = CB_INT8;
-	rc = cbgpu_rel_create(ctx, ng, ncols, types, NULL, &rel);
+	rc = cbgpu_rel_create(ctx, ng, ncols, types, NULL, &created);
 	if (rc)
 		return rc;
+	CbOwned<cbgpu_rel> rel(created, cbgpu_rel_free);
+
 	memset(&o, 0, sizeof(o));
 	int			blocks = (int) ((t->capacity + 255) / 256);
 
@@ -484,15 +484,14 @@ cbgpu_agg_to_rel(cbgpu_aggtable *t, const int32_t *keytypes, cbgpu_rel **out)
 	}
 	for (int a = 0; a < t->d.naccs * 3; a++)
 		o.acc[a] = (int64_t *) rel->data[t->d.nkeys + a];
-	CB_CUDA(ctx, cudaMallocAsync(&o.counter, sizeof(int32_t), ctx->stream));
+	CB_CUDA(ctx, mem.alloc(&o.counter, sizeof(int32_t)));
 	CB_CUDA(ctx, cudaMemsetAsync(o.counter, 0, sizeof(int32_t), ctx->stream));
 	if (ng > 0)
 	{
 		k_agg_to_rel<<<blocks, 256, 0, ctx->stream>>>(t->d, o);
 		CB_LAUNCHED(ctx, "k_agg_to_rel");
 	}
-	CB_CUDA(ctx, cudaFreeAsync(o.counter, ctx->stream));
-	*out = rel;
+	*out = rel.release();
 	return CBGPU_OK;
 }
 
@@ -841,6 +840,7 @@ extern "C" int
 cbgpu_merge_sorted_runs(cbgpu_ctx *ctx, cbgpu_rel *rel, const int32_t *keycols, const int32_t *descending, const int32_t *unsigned_cmp,
 						int32_t nkeys, int32_t max_runs, uint32_t **order_dev, int32_t *nruns_out)
 {
+	CbCallMem	mem(ctx);
 	MergeParams p;
 	int32_t		nfound = 0;
 	unsigned long long found[MERGE_MAXRUNS];
@@ -871,7 +871,7 @@ cbgpu_merge_sorted_runs(cbgpu_ctx *ctx, cbgpu_rel *rel, const int32_t *keycols, 
 	blocks = (int) ((rel->nrows + 255) / 256);
 	if (blocks > ctx->sm_count * 8)
 		blocks = ctx->sm_count * 8;
-	CB_CUDA(ctx, cudaMallocAsync(&p.nfound, sizeof(int32_t) + MERGE_MAXRUNS * sizeof(unsigned long long) + 8, ctx->stream));
+	CB_CUDA(ctx, mem.alloc(&p.nfound, sizeof(int32_t) + MERGE_MAXRUNS * sizeof(unsigned long long) + 8));
 	p.found = (unsigned long long *) ((char *) p.nfound + 8);
 	CB_CUDA(ctx, cudaMemsetAsync(p.nfound, 0, sizeof(int32_t), ctx->stream));
 	k_merge_find_runs<<<blocks, 256, 0, ctx->stream>>>(p);
@@ -879,7 +879,7 @@ cbgpu_merge_sorted_runs(cbgpu_ctx *ctx, cbgpu_rel *rel, const int32_t *keycols, 
 	CB_CUDA(ctx, cudaMemcpyAsync(&nfound, p.nfound, sizeof(int32_t), cudaMemcpyDeviceToHost, ctx->stream));
 	CB_CUDA(ctx, cudaMemcpyAsync(found, p.found, sizeof(found), cudaMemcpyDeviceToHost, ctx->stream));
 	CB_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-	CB_CUDA(ctx, cudaFreeAsync(p.nfound, ctx->stream));
+	CB_CUDA(ctx, mem.free(p.nfound));
 	if (nfound + 1 > max_runs)
 		return cb_fail(ctx, CBGPU_ERR_INVALID, "merge receive: %s%lld sorted runs arrived from fewer senders - a sender's stream is not in the Motion's sort order",
 					   "", (long long) nfound + 1);
@@ -901,10 +901,10 @@ cbgpu_merge_sorted_runs(cbgpu_ctx *ctx, cbgpu_rel *rel, const int32_t *keycols, 
 	for (int a = 0; a < nfound; a++)
 		p.start[a + 1] = (int64_t) found[a];
 	p.start[p.nruns] = rel->nrows;
-	CB_CUDA(ctx, cudaMallocAsync(&p.order, (size_t) rel->nrows * sizeof(uint32_t), ctx->stream));
+	CB_CUDA(ctx, mem.alloc(&p.order, (size_t) rel->nrows * sizeof(uint32_t)));
 	k_merge_place<<<blocks, 256, 0, ctx->stream>>>(p);
 	CB_LAUNCHED(ctx, "k_merge_place");
-	*order_dev = p.order;
+	*order_dev = mem.detach(p.order);
 	return CBGPU_OK;
 }
 
@@ -912,11 +912,12 @@ extern "C" int
 cbgpu_topn(cbgpu_ctx *ctx, cbgpu_rel *rel, const int32_t *keycols, const int32_t *descending, const int32_t *unsigned_cmp,
 		   int32_t nkeys, int64_t limit, uint32_t *host_idx, int64_t *nout)
 {
+	CbCallMem	mem(ctx);
 	TopnParams	p;
 	uint32_t   *cand1 = NULL,
 			   *cand2 = NULL;
-	int64_t		n1,
-				n2;
+	int64_t		n1;
+	bool		done = false;
 
 	if (nkeys < 1 || nkeys > TOPN_MAXKEYS || limit < 1 || limit > TOPN_MAXK)
 		return cb_fail(ctx, CBGPU_ERR_UNSUPPORTED, "device top-N supports 1..4 sort keys and LIMIT <= 64 (%s got %lld)", "", limit);
@@ -946,11 +947,10 @@ cbgpu_topn(cbgpu_ctx *ctx, cbgpu_rel *rel, const int32_t *keycols, const int32_t
 		int		   *ncand = NULL;
 		unsigned long long h3[3];
 		int			hn = 0;
-		bool		done = false;
 
 		p.in_idx = NULL;
 		p.nin = rel->nrows;
-		CB_CUDA(ctx, cudaMallocAsync(&cand1, (TOPN_MAXK + 1) * sizeof(uint32_t), ctx->stream));
+		CB_CUDA(ctx, mem.alloc(&cand1, (TOPN_MAXK + 1) * sizeof(uint32_t)));
 		if (rel->nrows <= TOPN_CAND)
 		{
 			k_topn_final<<<1, 1024, 0, ctx->stream>>>(p, NULL, NULL, rel->nrows, cand1);
@@ -970,9 +970,9 @@ cbgpu_topn(cbgpu_ctx *ctx, cbgpu_rel *rel, const int32_t *keycols, const int32_t
 				nblocks = TOPN_BLOCKS;
 			while (tpb > 64 && (int64_t) (nblocks - 1) * tpb >= rel->nrows)
 				tpb >>= 1;
-			CB_CUDA(ctx, cudaMallocAsync(&scratch, (2 * TOPN_BLOCKS + 3) * sizeof(unsigned long long), ctx->stream));
-			CB_CUDA(ctx, cudaMallocAsync(&cand, TOPN_CAND * sizeof(uint32_t), ctx->stream));
-			CB_CUDA(ctx, cudaMallocAsync(&ncand, sizeof(int), ctx->stream));
+			CB_CUDA(ctx, mem.alloc(&scratch, (2 * TOPN_BLOCKS + 3) * sizeof(unsigned long long)));
+			CB_CUDA(ctx, mem.alloc(&cand, TOPN_CAND * sizeof(uint32_t)));
+			CB_CUDA(ctx, mem.alloc(&ncand, sizeof(int)));
 			for (int keyi = 0; keyi < nkeys && !done; keyi++)
 			{
 				k_topn_min<<<nblocks, tpb, 0, ctx->stream>>>(p, keyi, scratch, scratch + TOPN_BLOCKS);
@@ -996,18 +996,15 @@ cbgpu_topn(cbgpu_ctx *ctx, cbgpu_rel *rel, const int32_t *keycols, const int32_t
 				}
 				break;			/* heavily tied key: the tournament sorts it out */
 			}
-			CB_CUDA(ctx, cudaFreeAsync(scratch, ctx->stream));
-			CB_CUDA(ctx, cudaFreeAsync(cand, ctx->stream));
-			CB_CUDA(ctx, cudaFreeAsync(ncand, ctx->stream));
+			CB_CUDA(ctx, mem.free(scratch));
+			CB_CUDA(ctx, mem.free(cand));
+			CB_CUDA(ctx, mem.free(ncand));
 		}
-		if (done)
-			goto fetch;
-		CB_CUDA(ctx, cudaFreeAsync(cand1, ctx->stream));
-		cand1 = NULL;
 	}
 	/* tournament: every pass gives each thread up to per_thread candidates and keeps its best k, until one
 	 * thread holds the answer.  per_thread >= 4k, so a pass leaves at most half its input (k per thread,
 	 * padded); a pass that does not shrink its input is an error, never an endless loop */
+	if (!done)
 	{
 		const int	threads = 128;
 		const int64_t per_thread = limit * 4 > 64 ? limit * 4 : 64;
@@ -1016,8 +1013,9 @@ cbgpu_topn(cbgpu_ctx *ctx, cbgpu_rel *rel, const int32_t *keycols, const int32_t
 		int			which = 0;
 		int64_t		cap = ((rel->nrows + per_thread - 1) / per_thread + threads) * limit;
 
-		CB_CUDA(ctx, cudaMallocAsync(&cand1, cap * sizeof(uint32_t), ctx->stream));
-		CB_CUDA(ctx, cudaMallocAsync(&cand2, cap * sizeof(uint32_t), ctx->stream));
+		CB_CUDA(ctx, mem.free(cand1));
+		CB_CUDA(ctx, mem.alloc(&cand1, cap * sizeof(uint32_t)));
+		CB_CUDA(ctx, mem.alloc(&cand2, cap * sizeof(uint32_t)));
 		for (;;)
 		{
 			int64_t		nthreads = (nin + per_thread - 1) / per_thread;
@@ -1043,22 +1041,14 @@ cbgpu_topn(cbgpu_ctx *ctx, cbgpu_rel *rel, const int32_t *keycols, const int32_t
 				break;
 			}
 			if (n1 >= nin)
-			{
-				cudaFreeAsync(cand1, ctx->stream);
-				cudaFreeAsync(cand2, ctx->stream);
 				return cb_fail(ctx, CBGPU_ERR_INVALID, "device top-N: a tournament pass did not shrink its input%s (%lld candidates)", "", nin);
-			}
 			in = outbuf;
 			nin = n1;
 			which ^= 1;
 		}
-		(void) n2;
 	}
-fetch:
 	CB_CUDA(ctx, cudaMemcpyAsync(host_idx, cand1, limit * sizeof(uint32_t), cudaMemcpyDeviceToHost, ctx->stream));
 	CB_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-	cudaFreeAsync(cand1, ctx->stream);
-	cudaFreeAsync(cand2, ctx->stream);
 	int64_t		n = 0;
 
 	while (n < limit && host_idx[n] != 0xFFFFFFFFu)

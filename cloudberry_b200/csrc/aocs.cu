@@ -1394,6 +1394,7 @@ aocs_decode_impl(cbgpu_ctx *ctx, const void *file_bytes, int64_t nbytes, int32_t
 				 const cbgpu_dict *dict, int dmode)
 {
 	const uint8_t *raw = (const uint8_t *) file_bytes;
+	CbCallMem	mem(ctx);
 	AocsDir    *dir = NULL;
 	AocsWalk	W;
 	int64_t		ndir = 0,
@@ -1429,7 +1430,7 @@ aocs_decode_impl(cbgpu_ctx *ctx, const void *file_bytes, int64_t nbytes, int32_t
 
 		if (rc)
 			return rc;
-		dir = W.dir;
+		dir = mem.keep(W.dir);
 		ndir = W.ndir;
 		rows = W.rows;
 		ztotal = W.ztotal;
@@ -1437,20 +1438,14 @@ aocs_decode_impl(cbgpu_ctx *ctx, const void *file_bytes, int64_t nbytes, int32_t
 		anynull = W.anynull;
 	}
 	if (dmode != 1 && (row_offset < 0 || row_offset + rows > rel->capacity))
-	{
-		free(dir);
 		return cb_fail(ctx, CBGPU_ERR_INVALID, "AOCS column file holds %s%lld rows: more than the relation has room for", "", rows);
-	}
 	if (ndir == 0)
-	{
-		free(dir);
 		return CBGPU_OK;
-	}
 	CB_CUDA(ctx, cudaSetDevice(ctx->device));
-	CB_CUDA(ctx, cudaMallocAsync(&d_raw, (size_t) ((nbytes + 15) / 16 * 16 + ztotal + 16), ctx->stream));
-	CB_CUDA(ctx, cudaMallocAsync(&d_dir, sizeof(AocsDir) * (size_t) ndir, ctx->stream));
-	CB_CUDA(ctx, cudaMemcpyAsync(d_raw, raw, (size_t) nbytes, cudaMemcpyHostToDevice, ctx->stream));
-	CB_CUDA(ctx, cudaMemcpyAsync(d_dir, dir, sizeof(AocsDir) * (size_t) ndir, cudaMemcpyHostToDevice, ctx->stream));
+	CB_CUDA(ctx, mem.alloc(&d_raw, (size_t) ((nbytes + 15) / 16 * 16 + ztotal + 16)));
+	CB_CUDA(ctx, mem.alloc(&d_dir, sizeof(AocsDir) * (size_t) ndir));
+	CB_CUDA(ctx, mem.copy_in(d_raw, raw, (size_t) nbytes));
+	CB_CUDA(ctx, mem.copy_in(d_dir, dir, sizeof(AocsDir) * (size_t) ndir));
 	if (ctx->trace_on)
 		cb_trace_mark(ctx, "aocs:h2d");
 	nblk = (int) ((ndir + AOCS_WARPS - 1) / AOCS_WARPS);
@@ -1466,17 +1461,17 @@ aocs_decode_impl(cbgpu_ctx *ctx, const void *file_bytes, int64_t nbytes, int32_t
 	{
 		int			flag = 0;
 
-		CB_CUDA(ctx, cudaMallocAsync(&d_flag, sizeof(int), ctx->stream));
+		CB_CUDA(ctx, mem.alloc(&d_flag, sizeof(int)));
 		CB_CUDA(ctx, cudaMemsetAsync(d_flag, 0, sizeof(int), ctx->stream));
 		if (compress_kind == CBGPU_AOCS_COMPRESS_ZSTD)
 		{
 			/* a literal scratch area per warp bounds the grid */
 			const int	zblk = nblk < ctx->sm_count * 4 ? nblk : ctx->sm_count * 4;
 
-			CB_CUDA(ctx, cudaMallocAsync(&d_scratch, (size_t) zblk * AOCS_WARPS * ZSTD_SCRATCH, ctx->stream));
+			CB_CUDA(ctx, mem.alloc(&d_scratch, (size_t) zblk * AOCS_WARPS * ZSTD_SCRATCH));
 			k_aocs_unzstd<<<zblk, AOCS_WARPS * 32, 0, ctx->stream>>>(d_raw, d_dir, (int) ndir, ctx->d_status, d_flag, d_scratch);
 			CB_LAUNCHED(ctx, "k_aocs_unzstd");
-			CB_CUDA(ctx, cudaFreeAsync(d_scratch, ctx->stream));
+			CB_CUDA(ctx, mem.free(d_scratch));
 		}
 		else
 		{
@@ -1487,23 +1482,17 @@ aocs_decode_impl(cbgpu_ctx *ctx, const void *file_bytes, int64_t nbytes, int32_t
 		{
 			/* whether an inflated block carries a NULL bitmap is only known now */
 			CB_CUDA(ctx, cudaMemcpyAsync(&flag, d_flag, sizeof(int), cudaMemcpyDeviceToHost, ctx->stream));
-			CB_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+			CB_CUDA(ctx, mem.sync());
 			anynull = flag != 0;
 		}
-		CB_CUDA(ctx, cudaFreeAsync(d_flag, ctx->stream));
+		CB_CUDA(ctx, mem.free(d_flag));
 	}
 	if (dmode != 1 && anynull && !rel->nulls[col])
 	{
 		int			rc = cbgpu_rel_add_nullmap(rel, col);
 
 		if (rc)
-		{
-			cudaStreamSynchronize(ctx->stream);
-			cudaFreeAsync(d_raw, ctx->stream);
-			cudaFreeAsync(d_dir, ctx->stream);
-			free(dir);
 			return rc;
-		}
 	}
 	memset(&P, 0, sizeof(P));
 	P.raw = d_raw;
@@ -1533,10 +1522,9 @@ aocs_decode_impl(cbgpu_ctx *ctx, const void *file_bytes, int64_t nbytes, int32_t
 	}
 	k_aocs_decode<<<nblk, AOCS_WARPS * 32, 0, ctx->stream>>>(P);
 	CB_LAUNCHED(ctx, "k_aocs_decode");
-	CB_CUDA(ctx, cudaStreamSynchronize(ctx->stream));	/* the caller's file buffer and `dir` are free again */
-	CB_CUDA(ctx, cudaFreeAsync(d_raw, ctx->stream));
-	CB_CUDA(ctx, cudaFreeAsync(d_dir, ctx->stream));
-	free(dir);
+	CB_CUDA(ctx, mem.sync());	/* the caller's file buffer and `dir` are free again */
+	CB_CUDA(ctx, mem.free(d_raw));
+	CB_CUDA(ctx, mem.free(d_dir));
 	*nrows_out = rows;
 	return cbgpu_check_status(ctx);
 }
@@ -1545,7 +1533,6 @@ aocs_decode_impl(cbgpu_ctx *ctx, const void *file_bytes, int64_t nbytes, int32_t
 extern "C" int
 cbgpu_dict_create(cbgpu_ctx *ctx, int32_t max_entries, int64_t arena_bytes, int32_t bpchar, cbgpu_dict **out)
 {
-	cbgpu_dict *d;
 	uint32_t	nslots = 64;
 
 	*out = NULL;
@@ -1553,7 +1540,8 @@ cbgpu_dict_create(cbgpu_ctx *ctx, int32_t max_entries, int64_t arena_bytes, int3
 		return cb_fail(ctx, CBGPU_ERR_INVALID, "cbgpu_dict_create: %s%lld entries", "", max_entries);
 	while (nslots < (uint32_t) max_entries * 2u)
 		nslots <<= 1;
-	d = (cbgpu_dict *) calloc(1, sizeof(*d));
+	CbOwned<cbgpu_dict> d((cbgpu_dict *) calloc(1, sizeof(cbgpu_dict)), cbgpu_dict_free);
+
 	if (!d)
 		return CBGPU_ERR_NOMEM;
 	d->ctx = ctx;
@@ -1567,7 +1555,7 @@ cbgpu_dict_create(cbgpu_ctx *ctx, int32_t max_entries, int64_t arena_bytes, int3
 	CB_CUDA(ctx, cudaMallocAsync(&d->d_arena, (size_t) arena_bytes + 16, ctx->stream));
 	CB_CUDA(ctx, cudaMallocAsync(&d->d_cursor, 2 * sizeof(unsigned long long), ctx->stream));
 	CB_CUDA(ctx, cudaMemsetAsync(d->d_cursor, 0, 2 * sizeof(unsigned long long), ctx->stream));
-	*out = d;
+	*out = d.release();
 	return CBGPU_OK;
 }
 
@@ -1577,9 +1565,12 @@ cbgpu_dict_free(cbgpu_dict *d)
 	if (!d)
 		return;
 	cudaSetDevice(d->ctx->device);
-	cudaFreeAsync(d->d_slots, d->ctx->stream);
-	cudaFreeAsync(d->d_arena, d->ctx->stream);
-	cudaFreeAsync(d->d_cursor, d->ctx->stream);
+	if (d->d_slots)
+		cudaFreeAsync(d->d_slots, d->ctx->stream);
+	if (d->d_arena)
+		cudaFreeAsync(d->d_arena, d->ctx->stream);
+	if (d->d_cursor)
+		cudaFreeAsync(d->d_cursor, d->ctx->stream);
 	if (d->d_hashes)
 		cudaFreeAsync(d->d_hashes, d->ctx->stream);
 	free(d->texts);
@@ -1619,7 +1610,10 @@ cbgpu_aocs_decode_dict_column(cbgpu_ctx *ctx, const void *file_bytes, int64_t nb
 	if (dict->n > 0)
 	{
 		if (rel->dict_hash[col] && rel->dict_n[col] > 0)
+		{
 			cudaFreeAsync(rel->dict_hash[col], ctx->stream);
+			rel->dict_hash[col] = NULL;
+		}
 		CB_CUDA(ctx, cudaMallocAsync(&rel->dict_hash[col], (size_t) dict->n * sizeof(uint32_t), ctx->stream));
 		CB_CUDA(ctx, cudaMemcpyAsync(rel->dict_hash[col], dict->d_hashes, (size_t) dict->n * sizeof(uint32_t), cudaMemcpyDeviceToDevice,
 									 ctx->stream));
@@ -1648,6 +1642,7 @@ extern "C" int
 cbgpu_dict_finalize(cbgpu_dict *d, int32_t *nentries)
 {
 	cbgpu_ctx  *ctx = d->ctx;
+	CbCallMem	mem(ctx);
 	DictSlot   *slots;
 	unsigned long long cur[2];
 	uint32_t   *hashes;
@@ -1668,18 +1663,14 @@ cbgpu_dict_finalize(cbgpu_dict *d, int32_t *nentries)
 	CB_CUDA(ctx, cudaSetDevice(ctx->device));
 	CB_CUDA(ctx, cudaMemcpyAsync(cur, d->d_cursor, sizeof(cur), cudaMemcpyDeviceToHost, ctx->stream));
 	CB_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-	slots = (DictSlot *) malloc(sizeof(DictSlot) * (size_t) d->nslots);
+	slots = mem.keep((DictSlot *) malloc(sizeof(DictSlot) * (size_t) d->nslots));
 	d->texts = (char *) malloc((size_t) cur[0] + 16);
 	d->sorted = (int32_t *) malloc(sizeof(int32_t) * (size_t) (cur[1] ? cur[1] : 1));
 	d->off = (uint32_t *) malloc(sizeof(uint32_t) * (size_t) (cur[1] ? cur[1] : 1));
 	d->len = (uint32_t *) malloc(sizeof(uint32_t) * (size_t) (cur[1] ? cur[1] : 1));
-	hashes = (uint32_t *) malloc(sizeof(uint32_t) * (size_t) (cur[1] ? cur[1] : 1));
+	hashes = mem.keep((uint32_t *) malloc(sizeof(uint32_t) * (size_t) (cur[1] ? cur[1] : 1)));
 	if (!slots || !d->texts || !d->sorted || !d->off || !d->len || !hashes)
-	{
-		free(slots);
-		free(hashes);
 		return CBGPU_ERR_NOMEM;
-	}
 	CB_CUDA(ctx, cudaMemcpyAsync(slots, d->d_slots, sizeof(DictSlot) * (size_t) d->nslots, cudaMemcpyDeviceToHost, ctx->stream));
 	CB_CUDA(ctx, cudaMemcpyAsync(d->texts, d->d_arena, (size_t) cur[0], cudaMemcpyDeviceToHost, ctx->stream));
 	CB_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
@@ -1687,11 +1678,7 @@ cbgpu_dict_finalize(cbgpu_dict *d, int32_t *nentries)
 		if (slots[i].tag)
 			d->sorted[n++] = (int32_t) i;
 	if ((unsigned long long) n != cur[1])
-	{
-		free(slots);
-		free(hashes);
 		return cb_fail(ctx, CBGPU_ERR_INVALID, "dictionary set holds %s%lld entries, its counter says otherwise", "", n);
-	}
 	g_dict_sort_slots = slots;
 	g_dict_sort_texts = d->texts;
 	qsort(d->sorted, (size_t) n, sizeof(int32_t), dict_slot_cmp);
@@ -1705,12 +1692,10 @@ cbgpu_dict_finalize(cbgpu_dict *d, int32_t *nentries)
 		/* hashbpchar over the blank-trimmed bytes == hashtext over the same bytes: both hash_any (utils/adt/varchar.c:981-1010) */
 		hashes[c] = pg_hash_bytes_host((const unsigned char *) d->texts + sl->off, (int) sl->len);
 	}
-	CB_CUDA(ctx, cudaMemcpyAsync(d->d_slots, slots, sizeof(DictSlot) * (size_t) d->nslots, cudaMemcpyHostToDevice, ctx->stream));
+	CB_CUDA(ctx, mem.copy_in(d->d_slots, slots, sizeof(DictSlot) * (size_t) d->nslots));
 	CB_CUDA(ctx, cudaMallocAsync(&d->d_hashes, sizeof(uint32_t) * (size_t) (n ? n : 1), ctx->stream));
-	CB_CUDA(ctx, cudaMemcpyAsync(d->d_hashes, hashes, sizeof(uint32_t) * (size_t) n, cudaMemcpyHostToDevice, ctx->stream));
-	CB_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-	free(slots);
-	free(hashes);
+	CB_CUDA(ctx, mem.copy_in(d->d_hashes, hashes, sizeof(uint32_t) * (size_t) n));
+	CB_CUDA(ctx, mem.sync());
 	d->n = n;
 	d->finalized = 1;
 	if (nentries)
@@ -1951,6 +1936,7 @@ extern "C" int
 cbgpu_aocs_apply_visimap(cbgpu_ctx *ctx, const void *file_bytes, int64_t nbytes, int32_t checksum, const cbgpu_visimap_entry *entries,
 						 int32_t nentries, cbgpu_rel *rel, int64_t row_offset, int64_t *nhidden_out)
 {
+	CbCallMem	mem(ctx);
 	AocsWalk	W;
 	VisiEntryDev *ent = NULL;
 	uint8_t    *blob = NULL;
@@ -1970,43 +1956,25 @@ cbgpu_aocs_apply_visimap(cbgpu_ctx *ctx, const void *file_bytes, int64_t nbytes,
 	rc = aocs_walk(ctx, (const uint8_t *) file_bytes, nbytes, checksum, -1, row_offset, &W);
 	if (rc)
 		return rc;
+	mem.keep(W.dir);
 	if (row_offset < 0 || row_offset + W.rows > rel->capacity)
-	{
-		free(W.dir);
 		return cb_fail(ctx, CBGPU_ERR_INVALID, "AOCS column file holds %s%lld rows: more than the relation has room for", "", W.rows);
-	}
 	for (int64_t i = 0; i < W.ndir; i++)
 		if (W.dir[i].first < 0)
-		{
-			free(W.dir);
 			return cb_fail(ctx, CBGPU_ERR_UNSUPPORTED, "AOCS block %s%lld carries no first row number: rows cannot be matched to visimap entries", "", i);
-		}
 	if (W.ndir == 0)
-	{
-		free(W.dir);
 		return CBGPU_OK;
-	}
-	ent = (VisiEntryDev *) malloc(sizeof(VisiEntryDev) * (size_t) (nentries ? nentries : 1));
+	ent = mem.keep((VisiEntryDev *) malloc(sizeof(VisiEntryDev) * (size_t) (nentries ? nentries : 1)));
 	for (int i = 0; i < nentries; i++)
 		blobsz += entries[i].data ? ((int64_t) entries[i].len + 7) / 8 * 8 : 0;
-	blob = (uint8_t *) calloc((size_t) blobsz + 8, 1);
+	blob = mem.keep((uint8_t *) calloc((size_t) blobsz + 8, 1));
 	if (!ent || !blob)
-	{
-		free(W.dir);
-		free(ent);
-		free(blob);
 		return CBGPU_ERR_NOMEM;
-	}
 	blobsz = 0;
 	for (int i = 0; i < nentries; i++)
 	{
 		if (entries[i].first_row_num < 0 || entries[i].first_row_num % VISIMAP_RANGE != 0 || (entries[i].data && entries[i].len < 6))
-		{
-			free(W.dir);
-			free(ent);
-			free(blob);
 			return cb_fail(ctx, CBGPU_ERR_INVALID, "visimap entry %s%lld: first row number is not a multiple of 32768, or the data is too short", "", i);
-		}
 		ent[i].first = entries[i].first_row_num;
 		ent[i].len = entries[i].data ? entries[i].len : 0;
 		ent[i].pad = 0;
@@ -2021,14 +1989,7 @@ cbgpu_aocs_apply_visimap(cbgpu_ctx *ctx, const void *file_bytes, int64_t nbytes,
 	qsort(ent, (size_t) nentries, sizeof(VisiEntryDev), visi_entry_cmp);
 	for (int i = 1; i < nentries; i++)
 		if (ent[i].first == ent[i - 1].first)
-		{
-			const long long twice = ent[i].first;
-
-			free(W.dir);
-			free(ent);
-			free(blob);
-			return cb_fail(ctx, CBGPU_ERR_INVALID, "two visimap entries for first row number %s%lld", "", twice);
-		}
+			return cb_fail(ctx, CBGPU_ERR_INVALID, "two visimap entries for first row number %s%lld", "", (long long) ent[i].first);
 	CB_CUDA(ctx, cudaSetDevice(ctx->device));
 	if (!rel->visimap)
 	{
@@ -2037,17 +1998,17 @@ cbgpu_aocs_apply_visimap(cbgpu_ctx *ctx, const void *file_bytes, int64_t nbytes,
 		CB_CUDA(ctx, cudaMallocAsync(&rel->visimap, ((bytes + 255) & ~(size_t) 255) + 256, ctx->stream));
 		CB_CUDA(ctx, cudaMemsetAsync(rel->visimap, 0xFF, ((bytes + 255) & ~(size_t) 255) + 256, ctx->stream));
 	}
-	CB_CUDA(ctx, cudaMallocAsync(&d_dir, sizeof(AocsDir) * (size_t) W.ndir, ctx->stream));
-	CB_CUDA(ctx, cudaMemcpyAsync(d_dir, W.dir, sizeof(AocsDir) * (size_t) W.ndir, cudaMemcpyHostToDevice, ctx->stream));
-	CB_CUDA(ctx, cudaMallocAsync(&d_cnt, sizeof(unsigned long long), ctx->stream));
+	CB_CUDA(ctx, mem.alloc(&d_dir, sizeof(AocsDir) * (size_t) W.ndir));
+	CB_CUDA(ctx, mem.copy_in(d_dir, W.dir, sizeof(AocsDir) * (size_t) W.ndir));
+	CB_CUDA(ctx, mem.alloc(&d_cnt, sizeof(unsigned long long)));
 	CB_CUDA(ctx, cudaMemsetAsync(d_cnt, 0, sizeof(unsigned long long), ctx->stream));
 	if (nentries)
 	{
-		CB_CUDA(ctx, cudaMallocAsync(&d_ent, sizeof(VisiEntryDev) * (size_t) nentries, ctx->stream));
-		CB_CUDA(ctx, cudaMemcpyAsync(d_ent, ent, sizeof(VisiEntryDev) * (size_t) nentries, cudaMemcpyHostToDevice, ctx->stream));
-		CB_CUDA(ctx, cudaMallocAsync(&d_blob, (size_t) blobsz + 8, ctx->stream));
-		CB_CUDA(ctx, cudaMemcpyAsync(d_blob, blob, (size_t) blobsz + 8, cudaMemcpyHostToDevice, ctx->stream));
-		CB_CUDA(ctx, cudaMallocAsync(&d_words, sizeof(uint32_t) * VISIMAP_WORDS * (size_t) nentries, ctx->stream));
+		CB_CUDA(ctx, mem.alloc(&d_ent, sizeof(VisiEntryDev) * (size_t) nentries));
+		CB_CUDA(ctx, mem.copy_in(d_ent, ent, sizeof(VisiEntryDev) * (size_t) nentries));
+		CB_CUDA(ctx, mem.alloc(&d_blob, (size_t) blobsz + 8));
+		CB_CUDA(ctx, mem.copy_in(d_blob, blob, (size_t) blobsz + 8));
+		CB_CUDA(ctx, mem.alloc(&d_words, sizeof(uint32_t) * VISIMAP_WORDS * (size_t) nentries));
 		k_visimap_expand<<<(nentries + 127) / 128, 128, 0, ctx->stream>>>(d_blob, d_ent, nentries, d_words, ctx->d_status);
 		CB_LAUNCHED(ctx, "k_visimap_expand");
 	}
@@ -2061,18 +2022,15 @@ cbgpu_aocs_apply_visimap(cbgpu_ctx *ctx, const void *file_bytes, int64_t nbytes,
 		CB_LAUNCHED(ctx, "k_visimap_apply");
 	}
 	CB_CUDA(ctx, cudaMemcpyAsync(&cnt, d_cnt, sizeof(cnt), cudaMemcpyDeviceToHost, ctx->stream));
-	CB_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-	CB_CUDA(ctx, cudaFreeAsync(d_dir, ctx->stream));
-	CB_CUDA(ctx, cudaFreeAsync(d_cnt, ctx->stream));
+	CB_CUDA(ctx, mem.sync());
+	CB_CUDA(ctx, mem.free(d_dir));
+	CB_CUDA(ctx, mem.free(d_cnt));
 	if (nentries)
 	{
-		CB_CUDA(ctx, cudaFreeAsync(d_ent, ctx->stream));
-		CB_CUDA(ctx, cudaFreeAsync(d_blob, ctx->stream));
-		CB_CUDA(ctx, cudaFreeAsync(d_words, ctx->stream));
+		CB_CUDA(ctx, mem.free(d_ent));
+		CB_CUDA(ctx, mem.free(d_blob));
+		CB_CUDA(ctx, mem.free(d_words));
 	}
-	free(W.dir);
-	free(ent);
-	free(blob);
 	if (nhidden_out)
 		*nhidden_out = (int64_t) cnt;
 	return cbgpu_check_status(ctx);

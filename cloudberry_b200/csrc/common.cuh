@@ -17,6 +17,8 @@
 #include <stdlib.h>
 #include <string.h>
 
+#include <memory>
+
 #define CB_MAX_COLS_REL 64
 
 struct cbgpu_ctx
@@ -320,6 +322,98 @@ void		cb_trace_mark(cbgpu_ctx *ctx, const char *name);
 			return CBGPU_ERR_CUDA; \
 		} \
 	} while (0)
+
+/* a constructor's object until it is handed out: CB_CUDA and CB_LAUNCHED return from the middle of a function, and on
+ * any early return the object goes through its own free function (which skips members never allocated) */
+template <typename T> using CbOwned = std::unique_ptr<T, void (*)(T *)>;
+
+/* the buffers one call allocates for its own duration: device buffers (stream-ordered on ctx->stream) and malloc'ed host
+ * buffers, freed when the call returns by whichever exit.  copy_in queues a copy from host memory; until sync() has
+ * waited for it, the destructor drains the stream first, so that the caller may free that memory once the call returns
+ * and the call's own host buffers are not freed under the copy.  A free that fails here is ignored: the call's error
+ * stands. */
+struct CbCallMem
+{
+	cbgpu_ctx  *ctx;
+	void	   *dev[16] = {};
+	void	   *host[4] = {};
+	int			ndev = 0,
+				nhost = 0;
+	bool		in_flight = false;
+
+	explicit	CbCallMem(cbgpu_ctx *c) : ctx(c) {}
+	CbCallMem(const CbCallMem &) = delete;
+	CbCallMem &operator=(const CbCallMem &) = delete;
+
+	~CbCallMem()
+	{
+		if (in_flight)
+			(void) cudaStreamSynchronize(ctx->stream);
+		for (int i = 0; i < ndev; i++)
+			if (dev[i] && cudaFreeAsync(dev[i], ctx->stream) != cudaSuccess)
+				(void) cudaGetLastError();
+		for (int i = 0; i < nhost; i++)
+			::free(host[i]);
+	}
+
+	template <typename T> cudaError_t
+	alloc(T **p, size_t bytes)
+	{
+		if (ndev == (int) (sizeof(dev) / sizeof(dev[0])))
+			return cudaErrorInvalidValue;
+		cudaError_t e = cudaMallocAsync((void **) p, bytes, ctx->stream);
+
+		if (e == cudaSuccess)
+			dev[ndev++] = *p;
+		return e;
+	}
+
+	/* a buffer freed before the call ends: where it frees today, so that peak memory stays as it is */
+	cudaError_t
+	free(void *p)
+	{
+		return cudaFreeAsync(detach(p), ctx->stream);
+	}
+
+	/* a buffer handed to the caller: no longer freed here */
+	template <typename T> T *
+	detach(T *p)
+	{
+		for (int i = 0; i < ndev; i++)
+			if (dev[i] == p)
+				dev[i] = NULL;
+		return p;
+	}
+
+	/* a malloc'ed host buffer (NULL when malloc failed), freed when the call returns */
+	template <typename T> T *
+	keep(T *p)
+	{
+		if (nhost == (int) (sizeof(host) / sizeof(host[0])))
+		{
+			::free(p);
+			return NULL;
+		}
+		return (T *) (host[nhost++] = p);
+	}
+
+	cudaError_t
+	copy_in(void *dst, const void *src, size_t bytes)
+	{
+		in_flight = true;
+		return cudaMemcpyAsync(dst, src, bytes, cudaMemcpyHostToDevice, ctx->stream);
+	}
+
+	cudaError_t
+	sync(void)
+	{
+		cudaError_t e = cudaStreamSynchronize(ctx->stream);
+
+		if (e == cudaSuccess)
+			in_flight = false;
+		return e;
+	}
+};
 
 int			cb_check_status(cbgpu_ctx *ctx, const char *what);	/* sync + read device status word */
 /* enqueue the status word's copy next to another device-to-host copy; call cb_status_fetched after the sync */

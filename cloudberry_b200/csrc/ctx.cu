@@ -22,15 +22,29 @@ cbgpu_device_count(void)
 	return n;
 }
 
+/* why this thread's last cbgpu_ctx_create failed: cbgpu_last_error(NULL) */
+static thread_local char create_err[sizeof(((cbgpu_ctx *) 0)->err)];
+
+static void
+ctx_create_failed(cbgpu_ctx *ctx)
+{
+	memcpy(create_err, ctx->err, sizeof(create_err));
+	cbgpu_ctx_destroy(ctx);
+}
+
 extern "C" int
 cbgpu_ctx_create(int device, cbgpu_ctx **out)
 {
-	cbgpu_ctx  *ctx = (cbgpu_ctx *) calloc(1, sizeof(cbgpu_ctx));
+	CbOwned<cbgpu_ctx> owned((cbgpu_ctx *) calloc(1, sizeof(cbgpu_ctx)), ctx_create_failed);
+	cbgpu_ctx  *ctx = owned.get();
 	cudaDeviceProp prop;
 
+	*out = NULL;
 	if (!ctx)
+	{
+		snprintf(create_err, sizeof(create_err), "cbgpu_ctx_create: out of host memory");
 		return CBGPU_ERR_NOMEM;
-	*out = ctx;
+	}
 	ctx->device = device;
 	CB_CUDA(ctx, cudaSetDevice(device));
 	CB_CUDA(ctx, cudaGetDeviceProperties(&prop, device));
@@ -63,6 +77,7 @@ cbgpu_ctx_create(int device, cbgpu_ctx **out)
 	/* L2 is 50 MB on H100: flush buffer comfortably larger */
 	ctx->flush_bytes = (size_t) 512 << 20;
 	ctx->flush_buf = NULL;
+	*out = owned.release();
 	return CBGPU_OK;
 }
 
@@ -71,29 +86,35 @@ cbgpu_ctx_destroy(cbgpu_ctx *ctx)
 {
 	if (!ctx)
 		return;
+	cudaEvent_t ev[] = {ctx->ev_t0, ctx->ev_t1, ctx->ev_k0, ctx->ev_k1};
+
 	cudaSetDevice(ctx->device);
-	cudaStreamSynchronize(ctx->stream);
+	if (ctx->stream)
+		cudaStreamSynchronize(ctx->stream);
 	if (ctx->flush_buf)
 		cudaFree(ctx->flush_buf);
-	cudaFree(ctx->d_status);
-	cudaFreeHost(ctx->h_status);
-	cudaFreeHost(ctx->agg_snap);
+	if (ctx->d_status)
+		cudaFree(ctx->d_status);
+	if (ctx->h_status)
+		cudaFreeHost(ctx->h_status);
+	if (ctx->agg_snap)
+		cudaFreeHost(ctx->agg_snap);
 	if (ctx->small_dev)
 		cudaFree(ctx->small_dev);
 	for (int i = 0; i < CB_SCRATCH_SLOTS; i++)
 		free(ctx->scratch[i]);
-	cudaEventDestroy(ctx->ev_t0);
-	cudaEventDestroy(ctx->ev_t1);
-	cudaEventDestroy(ctx->ev_k0);
-	cudaEventDestroy(ctx->ev_k1);
-	cudaStreamDestroy(ctx->stream);
+	for (int i = 0; i < 4; i++)
+		if (ev[i])
+			cudaEventDestroy(ev[i]);
+	if (ctx->stream)
+		cudaStreamDestroy(ctx->stream);
 	free(ctx);
 }
 
 extern "C" const char *
 cbgpu_last_error(cbgpu_ctx *ctx)
 {
-	return ctx ? ctx->err : "no context";
+	return ctx ? ctx->err : create_err[0] ? create_err : "no context";
 }
 
 extern "C" void
@@ -369,11 +390,11 @@ extern "C" int
 cbgpu_rel_create(cbgpu_ctx *ctx, int64_t nrows, int32_t ncols, const int32_t *types, const int32_t *dscales,
 				 cbgpu_rel **out)
 {
-	cbgpu_rel  *r;
-
+	*out = NULL;
 	if (ncols < 0 || ncols > CB_MAX_COLS_REL || nrows < 0 || nrows > 0xFFFFFFF0ll)
 		return cb_fail(ctx, CBGPU_ERR_INVALID, "cbgpu_rel_create: bad shape (%s nrows=%lld)", "", nrows);
-	r = (cbgpu_rel *) calloc(1, sizeof(cbgpu_rel));
+	CbOwned<cbgpu_rel> r((cbgpu_rel *) calloc(1, sizeof(cbgpu_rel)), cbgpu_rel_free);
+
 	if (!r)
 		return CBGPU_ERR_NOMEM;
 	r->ctx = ctx;
@@ -389,10 +410,7 @@ cbgpu_rel_create(cbgpu_ctx *ctx, int64_t nrows, int32_t ncols, const int32_t *ty
 		size_t		bytes = (size_t) (nrows ? nrows : 1) * cb_type_w(types[i]);
 
 		if (cb_type_w(types[i]) == 0)
-		{
-			free(r);
 			return cb_fail(ctx, CBGPU_ERR_INVALID, "cbgpu_rel_create: bad column type%s %lld", "", types[i]);
-		}
 		r->types[i] = types[i];
 		r->dscales[i] = dscales ? dscales[i] : 0;
 		/* pad so 16-byte vector loads and TMA bulk copies may read a whole final vector */
@@ -420,7 +438,7 @@ cbgpu_rel_create(cbgpu_ctx *ctx, int64_t nrows, int32_t ncols, const int32_t *ty
 			CB_CUDA(ctx, cudaMallocAsync(&r->data[i], colbytes[i], ctx->stream));
 			r->owns[i] = true;
 		}
-	*out = r;
+	*out = r.release();
 	return CBGPU_OK;
 }
 
@@ -514,6 +532,7 @@ extern "C" int
 cbgpu_rel_load_column_narrow(cbgpu_rel *rel, int32_t col, const void *host, int32_t host_width)
 {
 	cbgpu_ctx  *ctx = rel->ctx;
+	CbCallMem	mem(ctx);
 	void	   *stage;
 	int			w;
 	int			blocks;
@@ -527,7 +546,7 @@ cbgpu_rel_load_column_narrow(cbgpu_rel *rel, int32_t col, const void *host, int3
 		return cb_fail(ctx, CBGPU_ERR_INVALID, "cbgpu_rel_load_column_narrow: a %s%lld-byte host column cannot be widened into this column", "", host_width);
 	if (rel->nrows == 0)
 		return CBGPU_OK;
-	CB_CUDA(ctx, cudaMallocAsync(&stage, (size_t) rel->nrows * host_width, ctx->stream));
+	CB_CUDA(ctx, mem.alloc(&stage, (size_t) rel->nrows * host_width));
 	CB_CUDA(ctx, cudaMemcpyAsync(stage, host, (size_t) rel->nrows * host_width, cudaMemcpyHostToDevice, ctx->stream));
 	blocks = ctx->sm_count * 8;
 	if (w == 8)
@@ -547,7 +566,6 @@ cbgpu_rel_load_column_narrow(cbgpu_rel *rel, int32_t col, const void *host, int3
 			k_widen<int16_t, int32_t><<<blocks, 256, 0, ctx->stream>>>((const int16_t *) stage, (int32_t *) rel->data[col], rel->nrows);
 	}
 	CB_LAUNCHED(ctx, "k_widen");
-	CB_CUDA(ctx, cudaFreeAsync(stage, ctx->stream));
 	return CBGPU_OK;
 }
 
@@ -610,6 +628,7 @@ extern "C" int
 cbgpu_rel_read_rows(cbgpu_rel *rel, const uint32_t *host_idx, int64_t n, int64_t *out, uint8_t *outnull)
 {
 	cbgpu_ctx  *ctx = rel->ctx;
+	CbCallMem	mem(ctx);
 	ReadRows	p;
 	uint32_t   *d_idx = NULL;
 	char	   *d_buf = NULL;
@@ -632,13 +651,13 @@ cbgpu_rel_read_rows(cbgpu_rel *rel, const uint32_t *host_idx, int64_t n, int64_t
 	p.ncols = rel->ncols;
 	p.n = n;
 	CB_CUDA(ctx, cudaSetDevice(ctx->device));
-	CB_CUDA(ctx, cudaMallocAsync(&d_buf, (size_t) total * 9, ctx->stream));
+	CB_CUDA(ctx, mem.alloc(&d_buf, (size_t) total * 9));
 	p.out = (long long *) d_buf;
 	p.outnull = (uint8_t *) (d_buf + (size_t) total * 8);
 	if (host_idx)
 	{
-		CB_CUDA(ctx, cudaMallocAsync(&d_idx, (size_t) n * sizeof(uint32_t), ctx->stream));
-		CB_CUDA(ctx, cudaMemcpyAsync(d_idx, host_idx, (size_t) n * sizeof(uint32_t), cudaMemcpyHostToDevice, ctx->stream));
+		CB_CUDA(ctx, mem.alloc(&d_idx, (size_t) n * sizeof(uint32_t)));
+		CB_CUDA(ctx, mem.copy_in(d_idx, host_idx, (size_t) n * sizeof(uint32_t)));
 		p.idx = d_idx;
 	}
 	{
@@ -652,11 +671,8 @@ cbgpu_rel_read_rows(cbgpu_rel *rel, const uint32_t *host_idx, int64_t n, int64_t
 	CB_CUDA(ctx, cudaMemcpyAsync(out, p.out, (size_t) total * 8, cudaMemcpyDeviceToHost, ctx->stream));
 	CB_CUDA(ctx, cudaMemcpyAsync(outnull, p.outnull, (size_t) total, cudaMemcpyDeviceToHost, ctx->stream));
 	CB_CUDA(ctx, CB_STATUS_RIDE(ctx));
-	CB_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+	CB_CUDA(ctx, mem.sync());
 	CB_STATUS_FETCHED(ctx);
-	CB_CUDA(ctx, cudaFreeAsync(d_buf, ctx->stream));
-	if (d_idx)
-		CB_CUDA(ctx, cudaFreeAsync(d_idx, ctx->stream));
 	return CBGPU_OK;
 }
 
@@ -707,6 +723,7 @@ cbgpu_rel_set_dict_hash(cbgpu_rel *rel, int32_t col, const uint32_t *hashes, int
 	if (rel->dict_hash[col])
 	{
 		cudaFreeAsync(rel->dict_hash[col], ctx->stream);
+		rel->dict_hash[col] = NULL;
 	}
 	CB_CUDA(ctx, cudaMallocAsync(&rel->dict_hash[col], (size_t) n * sizeof(uint32_t), ctx->stream));
 	CB_CUDA(ctx, cudaMemcpyAsync(rel->dict_hash[col], hashes, (size_t) n * sizeof(uint32_t), cudaMemcpyHostToDevice, ctx->stream));

@@ -198,6 +198,7 @@ static int
 ht_create(cbgpu_ctx *ctx, cbgpu_rel *inner, const int32_t *keycols, int32_t nkeys, int32_t nbatch, cbgpu_hashtable **out)
 {
 	cbgpu_hashtable *ht;
+	CbCallMem	mem(ctx);
 	int64_t		nslots = 64;
 	int64_t		resident_rows = inner->nrows;
 
@@ -206,7 +207,8 @@ ht_create(cbgpu_ctx *ctx, cbgpu_rel *inner, const int32_t *keycols, int32_t nkey
 		return cb_fail(ctx, CBGPU_ERR_UNSUPPORTED, "hash join with %s%lld key columns is beyond the GPU path's limit (4)", "", nkeys);
 	if (nbatch < 1 || nbatch > 4096 || (nbatch & (nbatch - 1)) != 0)
 		return cb_fail(ctx, CBGPU_ERR_INVALID, "hash join with %s%lld batches (a power of two up to 4096 is expected)", "", nbatch);
-	ht = (cbgpu_hashtable *) calloc(1, sizeof(cbgpu_hashtable));
+	/* published at once: whatever fails from here on, cbgpu_ht_build frees it */
+	*out = ht = (cbgpu_hashtable *) calloc(1, sizeof(cbgpu_hashtable));
 	if (!ht)
 		return CBGPU_ERR_NOMEM;
 	ht->ctx = ctx;
@@ -222,20 +224,11 @@ ht_create(cbgpu_ctx *ctx, cbgpu_rel *inner, const int32_t *keycols, int32_t nkey
 		int			c = keycols[k];
 
 		if (c < 0 || c >= inner->ncols)
-		{
-			free(ht);
 			return cb_fail(ctx, CBGPU_ERR_INVALID, "cbgpu_ht_build: bad key column%s %lld", "", c);
-		}
 		if (inner->types[c] == CB_NUMERIC)
-		{
-			free(ht);
 			return cb_fail(ctx, CBGPU_ERR_UNSUPPORTED, "numeric hash join keys (hash_numeric) are not on the GPU path%s", "", 0);
-		}
 		if ((inner->types[c] == CB_DICT8 || inner->types[c] == CB_DICT32) && !inner->dict_hash[c])
-		{
-			free(ht);
 			return cb_fail(ctx, CBGPU_ERR_INVALID, "dictionary column %s%lld used as a join key without dict hashes", "", c);
-		}
 		ht->d.keydata[k] = inner->data[c];
 		ht->d.keynulls[k] = inner->nulls[c];
 		ht->d.keydict[k] = inner->dict_hash[c];
@@ -246,36 +239,29 @@ ht_create(cbgpu_ctx *ctx, cbgpu_rel *inner, const int32_t *keycols, int32_t nkey
 	{
 		/* the fullest batch sizes the table (hash skew: duplicate keys all land in one batch) */
 		unsigned long long *d_hist,
-				   *h_hist = (unsigned long long *) calloc((size_t) nbatch, sizeof(unsigned long long));
+				   *h_hist = mem.keep((unsigned long long *) calloc((size_t) nbatch, sizeof(unsigned long long)));
 		int			blocks = (int) ((inner->nrows + 255) / 256);
 
 		if (!h_hist)
-		{
-			free(ht);
 			return CBGPU_ERR_NOMEM;
-		}
 		if (blocks > ctx->sm_count * 8)
 			blocks = ctx->sm_count * 8;
-		CB_CUDA(ctx, cudaMallocAsync(&d_hist, sizeof(unsigned long long) * (size_t) nbatch, ctx->stream));
+		CB_CUDA(ctx, mem.alloc(&d_hist, sizeof(unsigned long long) * (size_t) nbatch));
 		CB_CUDA(ctx, cudaMemsetAsync(d_hist, 0, sizeof(unsigned long long) * (size_t) nbatch, ctx->stream));
 		k_ht_batch_histogram<<<blocks, 256, 0, ctx->stream>>>(ht->d, inner->nrows, d_hist);
 		CB_LAUNCHED(ctx, "k_ht_batch_histogram");
 		CB_CUDA(ctx, cudaMemcpyAsync(h_hist, d_hist, sizeof(unsigned long long) * (size_t) nbatch, cudaMemcpyDeviceToHost, ctx->stream));
 		CB_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-		CB_CUDA(ctx, cudaFreeAsync(d_hist, ctx->stream));
+		CB_CUDA(ctx, mem.free(d_hist));
 		resident_rows = 0;
 		for (int b = 0; b < nbatch; b++)
 			if ((int64_t) h_hist[b] > resident_rows)
 				resident_rows = (int64_t) h_hist[b];
-		free(h_hist);
 	}
 	while (nslots < resident_rows * 2)
 		nslots <<= 1;
 	if (nslots > (1ll << 32))
-	{
-		free(ht);
 		return cb_fail(ctx, CBGPU_ERR_UNSUPPORTED, "hash join build side too large for 32-bit slots%s (%lld rows)", "", inner->nrows);
-	}
 	ht->nslots = nslots;
 	ht->d.mask = (uint32_t) (nslots - 1);
 	CB_CUDA(ctx, cudaMallocAsync(&ht->d.slots, (size_t) nslots * sizeof(unsigned long long), ctx->stream));
@@ -304,7 +290,6 @@ ht_create(cbgpu_ctx *ctx, cbgpu_rel *inner, const int32_t *keycols, int32_t nkey
 		ht->d.bloom_mask = (uint32_t) (words - 1);
 		ht->built_bytes = nslots * 8 + words * 4;
 	}
-	*out = ht;
 	return CBGPU_OK;
 }
 
@@ -364,10 +349,12 @@ cbgpu_ht_free(cbgpu_hashtable *ht)
 	if (!ht)
 		return;
 	cudaSetDevice(ht->ctx->device);
-	cudaFreeAsync(ht->d.slots, ht->ctx->stream);
+	if (ht->d.slots)
+		cudaFreeAsync(ht->d.slots, ht->ctx->stream);
 	if (ht->d.bloom)
 		cudaFreeAsync(ht->d.bloom, ht->ctx->stream);
-	cudaFreeAsync(ht->d_flags, ht->ctx->stream);
+	if (ht->d_flags)
+		cudaFreeAsync(ht->d_flags, ht->ctx->stream);
 	free(ht);
 }
 
@@ -820,21 +807,24 @@ k_ht_partition_write(int64_t n, int32_t nbatch, int64_t chunk, const uint16_t *r
 	}
 }
 
-/* the device and host buffers of a pair probe: freed by cbgpu_ht_probe_pairs whatever the outcome */
+/* the device and host buffers of a pair probe: allocated through `mem`, freed whatever the outcome */
 struct PairProbe
 {
-	uint16_t   *rowbatch;		/* [n] each outer row's batch                                              */
-	unsigned long long *hist;	/* [nbatch][partition CTAs] row counts, then their exclusive scan          */
-	unsigned long long *d_offsets;	/* [nbatch + 1] where each batch's run starts in rows                  */
-	unsigned long long *h_offsets;
-	uint32_t   *rows;			/* [n] outer row ids grouped by batch                                       */
-	unsigned long long *counts;	/* match counts of one run (the last also of the build rows), then their scan */
-	uint8_t    *matched;		/* RIGHT / FULL: [inner rows], kept across all passes                       */
-	uint32_t   *decision;		/* SEMI / ANTI with a join filter: each row's decision in the current pass  */
-	CbpColumn  *fcols;			/* the join filter's columns and ops on the device                          */
-	CbpOp	   *fops;
-	uint32_t   *grow[2];		/* the output's next, larger arrays while they are being filled             */
-	int64_t		cap;			/* pairs the output arrays hold                                             */
+	CbCallMem	mem;
+	uint16_t   *rowbatch = NULL;	/* [n] each outer row's batch                                          */
+	unsigned long long *hist = NULL;	/* [nbatch][partition CTAs] row counts, then their exclusive scan      */
+	unsigned long long *d_offsets = NULL;	/* [nbatch + 1] where each batch's run starts in rows           */
+	unsigned long long *h_offsets = NULL;
+	uint32_t   *rows = NULL;		/* [n] outer row ids grouped by batch                                   */
+	unsigned long long *counts = NULL;	/* match counts of one run (the last also of the build rows), then their scan */
+	uint8_t    *matched = NULL;	/* RIGHT / FULL: [inner rows], kept across all passes                   */
+	uint32_t   *decision = NULL;	/* SEMI / ANTI with a join filter: each row's decision in the current pass */
+	CbpColumn  *fcols = NULL;	/* the join filter's columns and ops on the device                      */
+	CbpOp	   *fops = NULL;
+	uint32_t   *grow[2] = {};	/* the output's next, larger arrays while they are being filled (cudaMalloc: not in mem) */
+	int64_t		cap = 0;		/* pairs the output arrays hold                                         */
+
+	explicit	PairProbe(cbgpu_ctx *ctx) : mem(ctx) {}
 };
 
 /* the probe side's key columns of a pair probe */
@@ -921,10 +911,10 @@ join_filter_to_dev(cbgpu_ctx *ctx, const cbgpu_join_filter *jf, int32_t jointype
 	CB_CUDA(ctx, cudaSetDevice(ctx->device));
 	if (jf->ncols > 0)
 	{
-		CB_CUDA(ctx, cudaMallocAsync(&b->fcols, sizeof(CbpColumn) * (size_t) jf->ncols, ctx->stream));
+		CB_CUDA(ctx, b->mem.alloc(&b->fcols, sizeof(CbpColumn) * (size_t) jf->ncols));
 		CB_CUDA(ctx, cudaMemcpyAsync(b->fcols, jf->cols, sizeof(CbpColumn) * (size_t) jf->ncols, cudaMemcpyHostToDevice, ctx->stream));
 	}
-	CB_CUDA(ctx, cudaMallocAsync(&b->fops, sizeof(CbpOp) * (size_t) jf->nops, ctx->stream));
+	CB_CUDA(ctx, b->mem.alloc(&b->fops, sizeof(CbpOp) * (size_t) jf->nops));
 	CB_CUDA(ctx, cudaMemcpyAsync(b->fops, jf->ops, sizeof(CbpOp) * (size_t) jf->nops, cudaMemcpyHostToDevice, ctx->stream));
 	f->cols = b->fcols;
 	f->ops = b->fops;
@@ -1031,7 +1021,7 @@ ht_probe_batches(cbgpu_ctx *ctx, cbgpu_hashtable *ht, ProbeParams p, int fill_in
 	int			rc;
 
 	CB_CUDA(ctx, cudaSetDevice(ctx->device));
-	b->h_offsets = (unsigned long long *) calloc((size_t) nbatch + 1, sizeof(unsigned long long));
+	b->h_offsets = b->mem.keep((unsigned long long *) calloc((size_t) nbatch + 1, sizeof(unsigned long long)));
 	if (!b->h_offsets)
 		return cb_fail(ctx, CBGPU_ERR_NOMEM, "host memory for %s%lld batch offsets", "", nbatch);
 	if (nbatch == 1)
@@ -1048,10 +1038,10 @@ ht_probe_batches(cbgpu_ctx *ctx, cbgpu_hashtable *ht, ProbeParams p, int fill_in
 		if (grid > (n + HT_PART_THREADS - 1) / HT_PART_THREADS)
 			grid = (n + HT_PART_THREADS - 1) / HT_PART_THREADS;
 		chunk = (n + grid - 1) / grid;
-		CB_CUDA(ctx, cudaMallocAsync(&b->rowbatch, (size_t) n * sizeof(uint16_t), ctx->stream));
-		CB_CUDA(ctx, cudaMallocAsync(&b->hist, ((size_t) nbatch * grid + 1) * sizeof(unsigned long long), ctx->stream));
-		CB_CUDA(ctx, cudaMallocAsync(&b->d_offsets, ((size_t) nbatch + 1) * sizeof(unsigned long long), ctx->stream));
-		CB_CUDA(ctx, cudaMallocAsync(&b->rows, (size_t) n * sizeof(uint32_t), ctx->stream));
+		CB_CUDA(ctx, b->mem.alloc(&b->rowbatch, (size_t) n * sizeof(uint16_t)));
+		CB_CUDA(ctx, b->mem.alloc(&b->hist, ((size_t) nbatch * grid + 1) * sizeof(unsigned long long)));
+		CB_CUDA(ctx, b->mem.alloc(&b->d_offsets, ((size_t) nbatch + 1) * sizeof(unsigned long long)));
+		CB_CUDA(ctx, b->mem.alloc(&b->rows, (size_t) n * sizeof(uint32_t)));
 		k_ht_partition_count<<<(int) grid, HT_PART_THREADS, shmem, ctx->stream>>>(p, chunk, b->rowbatch, b->hist);
 		CB_LAUNCHED(ctx, "k_ht_partition_count");
 		k_exclusive_scan_u64<<<1, 1024, 0, ctx->stream>>>(b->hist, nbatch * grid);
@@ -1066,16 +1056,16 @@ ht_probe_batches(cbgpu_ctx *ctx, cbgpu_hashtable *ht, ProbeParams p, int fill_in
 	for (int32_t k = 0; k < nbatch; k++)
 		if ((int64_t) (b->h_offsets[k + 1] - b->h_offsets[k]) > maxrun)
 			maxrun = (int64_t) (b->h_offsets[k + 1] - b->h_offsets[k]);
-	CB_CUDA(ctx, cudaMallocAsync(&b->counts, (size_t) (maxrun + ninner + 1) * sizeof(unsigned long long), ctx->stream));
+	CB_CUDA(ctx, b->mem.alloc(&b->counts, (size_t) (maxrun + ninner + 1) * sizeof(unsigned long long)));
 	p.counts = b->counts;
 	if (p.f.ops && p.f.jointype != CB_JOIN_LEFT && maxrun)
 	{
-		CB_CUDA(ctx, cudaMallocAsync(&b->decision, (size_t) maxrun * sizeof(uint32_t), ctx->stream));
+		CB_CUDA(ctx, b->mem.alloc(&b->decision, (size_t) maxrun * sizeof(uint32_t)));
 		p.f.decision = b->decision;
 	}
 	if (ninner)
 	{
-		CB_CUDA(ctx, cudaMallocAsync(&b->matched, (size_t) ninner, ctx->stream));
+		CB_CUDA(ctx, b->mem.alloc(&b->matched, (size_t) ninner));
 		CB_CUDA(ctx, cudaMemsetAsync(b->matched, 0, (size_t) ninner, ctx->stream));
 		p.matched = b->matched;
 	}
@@ -1129,13 +1119,12 @@ cbgpu_ht_probe_pairs(cbgpu_ctx *ctx, cbgpu_hashtable *ht, cbgpu_rel *outer, cons
 {
 	const bool	taken = filter ? jointype == CB_JOIN_LEFT || jointype == CB_JOIN_SEMI || jointype == CB_JOIN_ANTI
 		: jointype == CB_JOIN_INNER || jointype == CB_JOIN_LEFT || jointype == CB_JOIN_RIGHT || jointype == CB_JOIN_FULL;
-	PairProbe	b;
+	PairProbe	b(ctx);
 	ProbeParams p;
 	int64_t		npasses = 0;
 	int			rc;
 
 	memset(out, 0, sizeof(*out));
-	memset(&b, 0, sizeof(b));
 	if (!taken)
 		rc = cb_fail(ctx, CBGPU_ERR_INVALID, "cbgpu_ht_probe_pairs: join type %s%lld (INNER, LEFT, RIGHT or FULL without a join "
 					 "filter, LEFT, SEMI or ANTI with one)", "", jointype);
@@ -1153,17 +1142,9 @@ cbgpu_ht_probe_pairs(cbgpu_ctx *ctx, cbgpu_hashtable *ht, cbgpu_rel *outer, cons
 		rc = cb_check_status(ctx, "join filter");	/* integer overflow inside the filter */
 	if (passes)
 		*passes = npasses;
-	{
-		void	   *dev[] = {b.rowbatch, b.hist, b.d_offsets, b.rows, b.counts, b.matched, b.decision, b.fcols, b.fops};
-
-		for (size_t k = 0; k < sizeof(dev) / sizeof(dev[0]); k++)
-			if (dev[k])
-				cudaFreeAsync(dev[k], ctx->stream);
-	}
 	for (int k = 0; k < 2; k++)
 		if (b.grow[k])
 			cudaFree(b.grow[k]);
-	free(b.h_offsets);
 	if (rc != CBGPU_OK)
 		cbgpu_pairs_free(out);
 	return rc;

@@ -1621,7 +1621,7 @@ cb_try_probe_chain(cbgpu_ctx *ctx, const CbPipeline *p, const PipeDev *d, bool *
 	 * side: the build rows that also survive the later probes keyed only by that build side's columns (a dimension
 	 * joined to its sub-dimension further up the plan).  Rows of the scan that miss it are dropped before the first
 	 * hash-table access instead of after several. */
-	void	   *early_mem[PC_MAXEARLY] = {NULL, NULL};
+	CbCallMem	mem(ctx);
 
 	for (int k = 0; k < np && P.nearly < PC_MAXEARLY; k++)
 	{
@@ -1677,7 +1677,7 @@ cb_try_probe_chain(cbgpu_ctx *ctx, const CbPipeline *p, const PipeDev *d, bool *
 					known = ctx->early_cache[i].worth;
 			if (known < 0)
 			{
-				CB_CUDA(ctx, cudaMallocAsync(&d_passed, sizeof(*d_passed), ctx->stream));
+				CB_CUDA(ctx, mem.alloc(&d_passed, sizeof(*d_passed)));
 				CB_CUDA(ctx, cudaMemsetAsync(d_passed, 0, sizeof(*d_passed), ctx->stream));
 				B.nrows = sample;
 				B.self = q->ht;
@@ -1689,7 +1689,7 @@ cb_try_probe_chain(cbgpu_ctx *ctx, const CbPipeline *p, const PipeDev *d, bool *
 				CB_LAUNCHED(ctx, "k_pc_early_build");
 				CB_CUDA(ctx, cudaMemcpyAsync(&h_passed, d_passed, sizeof(h_passed), cudaMemcpyDeviceToHost, ctx->stream));
 				CB_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-				CB_CUDA(ctx, cudaFreeAsync(d_passed, ctx->stream));
+				CB_CUDA(ctx, mem.free(d_passed));
 				known = (int64_t) h_passed * 2 <= sample;
 				{
 					const int	slot = ctx->early_cache_n < CB_EARLY_CACHE ? ctx->early_cache_n++ : (int) (inner->nrows % CB_EARLY_CACHE);
@@ -1705,13 +1705,12 @@ cb_try_probe_chain(cbgpu_ctx *ctx, const CbPipeline *p, const PipeDev *d, bool *
 		}
 		while (words < inner->nrows / 2)
 			words <<= 1;
-		CB_CUDA(ctx, cudaMallocAsync(&early_mem[P.nearly], (size_t) words * sizeof(uint32_t), ctx->stream));
-		CB_CUDA(ctx, cudaMemsetAsync(early_mem[P.nearly], 0, (size_t) words * sizeof(uint32_t), ctx->stream));
+		CB_CUDA(ctx, mem.alloc(&B.bloom, (size_t) words * sizeof(uint32_t)));
+		CB_CUDA(ctx, cudaMemsetAsync(B.bloom, 0, (size_t) words * sizeof(uint32_t), ctx->stream));
 		B.nrows = inner->nrows;
 		B.self = q->ht;
 		B.kc = kc;
 		B.hashtype = q->keytype[kc];
-		B.bloom = (uint32_t *) early_mem[P.nearly];
 		B.mask = (uint32_t) (words - 1);
 		{
 			int			eb = (int) ((inner->nrows + 255) / 256);
@@ -1776,8 +1775,8 @@ cb_try_probe_chain(cbgpu_ctx *ctx, const CbPipeline *p, const PipeDev *d, bool *
 			unsigned long long nsel = 0;
 			const int64_t ft = (P.nrows + PC_TILE - 1) / PC_TILE;
 
-			CB_CUDA(ctx, cudaMallocAsync(&pf_sel, (size_t) P.nrows * sizeof(uint32_t), ctx->stream));
-			CB_CUDA(ctx, cudaMallocAsync(&pf_count, sizeof(unsigned long long), ctx->stream));
+			CB_CUDA(ctx, mem.alloc(&pf_sel, (size_t) P.nrows * sizeof(uint32_t)));
+			CB_CUDA(ctx, mem.alloc(&pf_count, sizeof(unsigned long long)));
 			CB_CUDA(ctx, cudaMemsetAsync(pf_count, 0, sizeof(unsigned long long), ctx->stream));
 			F.out = pf_sel;
 			F.out_count = pf_count;
@@ -1860,7 +1859,7 @@ cb_try_probe_chain(cbgpu_ctx *ctx, const CbPipeline *p, const PipeDev *d, bool *
 		words += (int64_t) P.q_cap[k] * ((k + 3) / 2);
 	}
 	P.q_cta_words = words;
-	CB_CUDA(ctx, cudaMallocAsync(&P.qmem, (size_t) blocks * (size_t) (words ? words : 1) * sizeof(uint32_t), ctx->stream));
+	CB_CUDA(ctx, mem.alloc(&P.qmem, (size_t) blocks * (size_t) (words ? words : 1) * sizeof(uint32_t)));
 	if (ctx->opt_debug)
 		fprintf(stderr, "k_probe_chain: modes %d %d %d %d (0 filter + HBM table, 1 table only, 2 table in shared memory: %u bytes) fuse0 %d\n",
 				P.probe[0].mode, P.probe[1].mode, P.probe[2].mode, P.probe[3].mode, P.smem_table_bytes, P.fuse0);
@@ -1889,14 +1888,13 @@ cb_try_probe_chain(cbgpu_ctx *ctx, const CbPipeline *p, const PipeDev *d, bool *
 	CB_LAUNCHED(ctx, "k_probe_chain");
 	cb_klog_end(ctx, kl);
 	CB_CUDA(ctx, cudaEventRecord(ctx->ev_k1, ctx->stream));
-	CB_CUDA(ctx, cudaFreeAsync(P.qmem, ctx->stream));
+	/* queues, survivors, then the scan-level filters: the order blocks go back to the pool decides where the next run's
+	 * buffers land */
+	CB_CUDA(ctx, mem.free(P.qmem));
 	if (pf_sel)
-		CB_CUDA(ctx, cudaFreeAsync(pf_sel, ctx->stream));
+		CB_CUDA(ctx, mem.free(pf_sel));
 	if (pf_count)
-		CB_CUDA(ctx, cudaFreeAsync(pf_count, ctx->stream));
-	for (int f = 0; f < PC_MAXEARLY; f++)
-		if (early_mem[f])
-			CB_CUDA(ctx, cudaFreeAsync(early_mem[f], ctx->stream));
+		CB_CUDA(ctx, mem.free(pf_count));
 	ctx->kernel_timed = true;
 	*handled = true;
 	return CBGPU_OK;

@@ -9,6 +9,12 @@
  * (the reference reports errors with ereport(ERROR) = siglongjmp, utils/elog.h:185; the shim turns
  * a status code into ereport only after the stream is drained and device memory released).
  *
+ * A call that returns an error holds nothing it allocated, so that a caller that answers CBGPU_ERR_NOMEM by leaving
+ * the work to the CPU finds the device as it was, and a constructor (*_create, cbgpu_ht_build, cbgpu_agg_to_rel) leaves
+ * *out NULL.  The exception is state attached to an argument that outlives the call, which its owner frees: a NULL
+ * map, dictionary hashes or a visibility map added to a relation that was passed in.  Motion set-up
+ * (cbgpu_motion_create*) is outside this rule.
+ *
  * What each group of entry points replaces in the reference (paths under /root/reference/src):
  *
  *   relations / columns   the decoded form of an AOCS scan: aocs_beginscan (backend/access/aocs/
@@ -67,7 +73,7 @@ typedef struct cbgpu_motion cbgpu_motion;
  * ------------------------------------------------------------------------------------------ */
 int			cbgpu_ctx_create(int device, cbgpu_ctx **out);	/* lazily initialises CUDA: call after fork */
 void		cbgpu_ctx_destroy(cbgpu_ctx *ctx);
-const char *cbgpu_last_error(cbgpu_ctx *ctx);
+const char *cbgpu_last_error(cbgpu_ctx *ctx);	/* NULL: why this thread's last failed cbgpu_ctx_create failed */
 int			cbgpu_sync(cbgpu_ctx *ctx);						/* drain the context's stream              */
 /* drain the stream and report (then clear) an error a kernel raised: overflow, full table / buffer */
 int			cbgpu_check_status(cbgpu_ctx *ctx);
@@ -341,7 +347,7 @@ typedef struct cbgpu_join_filter
  * the last batch it loaded (nbatch - 1 after a success).  CBGPU_ERR_INVALID, before any launch, for a join type the call
  * does not take with (or without) a filter, or a malformed filter (a column src other than 0 / 1, a column or op outside the
  * supported set, a stack deeper than CBP_STACK, a program that does not leave exactly one value); CBGPU_ERR_OVERFLOW when
- * the filter's integer arithmetic overflows on a pair.  On failure *out is empty and nothing stays allocated. */
+ * the filter's integer arithmetic overflows on a pair.  On failure *out is empty. */
 int			cbgpu_ht_probe_pairs(cbgpu_ctx *ctx, cbgpu_hashtable *ht, cbgpu_rel *outer, const int32_t *keycols, int32_t nkeys,
 								 int32_t jointype, const cbgpu_join_filter *filter, int (*interrupted) (void *arg), void *arg,
 								 cbgpu_pairs *out, int64_t *passes);
