@@ -56,7 +56,7 @@ struct cbgpu_ctx
 	int			opt_bloom_div;
 	/* host-side scratch of the launch path (decompiled programs, kernel parameter blocks: too large for the
 	 * stack), owned by the context so that two contexts on two threads never share any: slot -> malloc'ed block */
-#define CB_SCRATCH_SLOTS 7
+#define CB_SCRATCH_SLOTS 6
 	void	   *scratch[CB_SCRATCH_SLOTS];
 	size_t		scratch_bytes[CB_SCRATCH_SLOTS];
 	/* scan-level runtime filter decisions, remembered per (build relation, rows, key column): the sample that

@@ -15,6 +15,7 @@
  */
 #include "common.cuh"
 #include "pipeline.cuh"
+#include "xmatch.h"
 
 #include <stdlib.h>
 
@@ -853,8 +854,11 @@ probe_params(cbgpu_ctx *ctx, const cbgpu_hashtable *ht, cbgpu_rel *outer, const 
 static int
 join_filter_to_dev(cbgpu_ctx *ctx, const cbgpu_join_filter *jf, int32_t jointype, PairProbe *b, JoinFilterDev *f)
 {
-	int			depth = 0;
+	XProg	   *x = (XProg *) cb_scratch(ctx, 2, sizeof(XProg));	/* the pipeline's slot: the two calls never overlap */
+	const XAllow allow = {"join filter", XM_SCALAR_OPS, NULL, 0, CBGPU_ERR_INVALID};
 
+	if (!x)
+		return CBGPU_ERR_NOMEM;
 	if (jf->ncols < 0 || jf->ncols > CBP_MAX_COLS || (jf->ncols > 0 && !jf->cols))
 		return cb_fail(ctx, CBGPU_ERR_INVALID, "join filter with %s%lld columns (0 .. 40 expected)", "", jf->ncols);
 	if (jf->nops < 1 || jf->nops > CBP_MAX_OPS || !jf->ops)
@@ -868,46 +872,12 @@ join_filter_to_dev(cbgpu_ctx *ctx, const cbgpu_join_filter *jf, int32_t jointype
 		if (c->type < CB_INT4 || c->type > CB_BOOL || !c->data)
 			return cb_fail(ctx, CBGPU_ERR_INVALID, "join filter column %s%lld: no data, or a type the filter cannot load", "", k);
 	}
-	for (int pc = 0; pc < jf->nops; pc++)
-	{
-		const CbpOp *op = &jf->ops[pc];
-		int			pops = 0;
+	int			rc = xm_walk(ctx, allow, jf->ncols, jf->ops, jf->nops, x);
 
-		switch (op->code)
-		{
-			case CBP_LOAD:
-				if (op->a < 0 || op->a >= jf->ncols)
-					return cb_fail(ctx, CBGPU_ERR_INVALID, "join filter op %s%lld loads a column it does not have", "", pc);
-				break;
-			case CBP_CONST:
-				break;
-			case CBP_DUP:
-				if (op->a < 0 || op->a >= depth)
-					return cb_fail(ctx, CBGPU_ERR_INVALID, "join filter op %s%lld copies a stack entry that is not there", "", pc);
-				break;
-			case CBP_POP:
-				pops = 1;
-				break;
-			case CBP_I2F: case CBP_F8ORD: case CBP_NOT:
-				pops = 1;
-				break;
-			case CBP_ADD: case CBP_SUB: case CBP_MUL: case CBP_FADD: case CBP_FSUB: case CBP_FMUL:
-			case CBP_EQ: case CBP_NE: case CBP_LT: case CBP_LE: case CBP_GT: case CBP_GE:
-			case CBP_FEQ: case CBP_FNE: case CBP_FLT: case CBP_FLE: case CBP_FGT: case CBP_FGE:
-			case CBP_AND: case CBP_OR:
-				pops = 2;
-				break;
-			default:
-				return cb_fail(ctx, CBGPU_ERR_INVALID, "join filter op %s%lld: opcode not supported in a join filter", "", pc);
-		}
-		if (depth < pops)
-			return cb_fail(ctx, CBGPU_ERR_INVALID, "join filter op %s%lld takes more values than the stack holds", "", pc);
-		depth += (op->code == CBP_POP ? 0 : 1) - pops;
-		if (depth > CBP_STACK)
-			return cb_fail(ctx, CBGPU_ERR_INVALID, "join filter stack deeper than %s%lld values", "", CBP_STACK);
-	}
-	if (depth != 1)
-		return cb_fail(ctx, CBGPU_ERR_INVALID, "join filter leaves %s%lld values (one expected)", "", depth);
+	if (rc != CBGPU_OK)
+		return rc;
+	if (x->depth != 1)
+		return cb_fail(ctx, CBGPU_ERR_INVALID, "join filter leaves %s%lld values (one expected)", "", x->depth);
 	CB_CUDA(ctx, cudaSetDevice(ctx->device));
 	if (jf->ncols > 0)
 	{

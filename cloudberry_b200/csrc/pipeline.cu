@@ -16,14 +16,15 @@
  * shape they fuse by hand; results are identical (tests run both).
  */
 #include "pipeline.cuh"
+#include "xmatch.h"
 
 #include <stdlib.h>
 
 /* ---------------------------------------------------------------------------------------------
- * host: descriptor -> device form
+ * host: descriptor -> device form, and the program's expression trees in *xp
  * --------------------------------------------------------------------------------------------- */
 int
-cb_pipeline_to_dev(cbgpu_ctx *ctx, const CbPipeline *p, PipeDev *d)
+cb_pipeline_to_dev(cbgpu_ctx *ctx, const CbPipeline *p, PipeDev *d, XProg *xp)
 {
 	memset(d, 0, sizeof(*d));
 	if (p->nrows < 0 || p->nrows > 0xFFFFFFF0ll)
@@ -44,60 +45,13 @@ cb_pipeline_to_dev(cbgpu_ctx *ctx, const CbPipeline *p, PipeDev *d)
 			return cb_fail(ctx, CBGPU_ERR_INVALID, "pipeline column %s%lld malformed", "", c);
 	}
 	d->nops = p->nops;
-	/* validate the program by simulating its stack depth */
-	int			depth = 0;
-
-	for (int i = 0; i < p->nops; i++)
+	memcpy(d->ops, p->ops, sizeof(CbpOp) * (size_t) p->nops);
 	{
-		const CbpOp *op = &p->ops[i];
+		const XAllow allow = {"pipeline", XM_PIPELINE_OPS, p->probes, p->nprobes, CBGPU_ERR_UNSUPPORTED};
+		const int	rc = xm_walk(ctx, allow, p->ncols, p->ops, p->nops, xp);
 
-		d->ops[i] = *op;
-		switch (op->code)
-		{
-			case CBP_LOAD:
-				if (op->a < 0 || op->a >= p->ncols)
-					return cb_fail(ctx, CBGPU_ERR_INVALID, "pipeline op %s%lld loads a missing column", "", i);
-				depth++;
-				break;
-			case CBP_CONST:
-				depth++;
-				break;
-			case CBP_DUP:
-				if (op->a < 0 || op->a >= depth)
-					return cb_fail(ctx, CBGPU_ERR_INVALID, "pipeline op %s%lld: DUP out of range", "", i);
-				depth++;
-				break;
-			case CBP_ADD: case CBP_SUB: case CBP_MUL: case CBP_FADD: case CBP_FSUB: case CBP_FMUL:
-			case CBP_EQ: case CBP_NE: case CBP_LT: case CBP_LE: case CBP_GT: case CBP_GE:
-			case CBP_FEQ: case CBP_FNE: case CBP_FLT: case CBP_FLE: case CBP_FGT: case CBP_FGE:
-			case CBP_AND: case CBP_OR:
-				if (depth < 2)
-					return cb_fail(ctx, CBGPU_ERR_INVALID, "pipeline op %s%lld underflows the stack", "", i);
-				depth--;
-				break;
-			case CBP_NOT: case CBP_I2F: case CBP_F8ORD:
-				if (depth < 1)
-					return cb_fail(ctx, CBGPU_ERR_INVALID, "pipeline op %s%lld underflows the stack", "", i);
-				break;
-			case CBP_FILTER: case CBP_POP:
-				if (depth < 1)
-					return cb_fail(ctx, CBGPU_ERR_INVALID, "pipeline op %s%lld underflows the stack", "", i);
-				depth--;
-				break;
-			case CBP_PROBE:
-				if (op->a < 0 || op->a >= p->nprobes || depth < p->probes[op->a].nkeys)
-					return cb_fail(ctx, CBGPU_ERR_INVALID, "pipeline op %s%lld: bad PROBE", "", i);
-				depth -= p->probes[op->a].nkeys;
-				break;
-			case CBP_END:
-				if (i != p->nops - 1)
-					return cb_fail(ctx, CBGPU_ERR_INVALID, "pipeline op %s%lld: END before the last op", "", i);
-				break;
-			default:
-				return cb_fail(ctx, CBGPU_ERR_INVALID, "pipeline op %s%lld: unknown opcode", "", i);
-		}
-		if (depth > CBP_STACK)
-			return cb_fail(ctx, CBGPU_ERR_UNSUPPORTED, "pipeline expression stack deeper than %s%lld", "", CBP_STACK);
+		if (rc != CBGPU_OK)
+			return rc;
 	}
 	if (p->ops[p->nops - 1].code != CBP_END)
 		return cb_fail(ctx, CBGPU_ERR_INVALID, "pipeline program does not end with END%s", "", 0);
@@ -146,7 +100,7 @@ cb_pipeline_to_dev(cbgpu_ctx *ctx, const CbPipeline *p, PipeDev *d)
 					return cb_fail(ctx, CBGPU_ERR_UNSUPPORTED, "numeric GROUP BY keys (hash_numeric) are not on the GPU path%s", "", 0);
 			}
 			{
-				int			nargs = depth - s->nkeys;
+				int			nargs = xp->depth - s->nkeys;
 
 				for (int a = 0; a < s->naccs; a++)
 				{
@@ -164,8 +118,8 @@ cb_pipeline_to_dev(cbgpu_ctx *ctx, const CbPipeline *p, PipeDev *d)
 			break;
 		case CBP_SINK_MATERIALIZE:
 		case CBP_SINK_PARTITION:
-			if (!s->out || s->nout != depth || s->nout > CBP_MAX_OUT || s->nout > s->out->ncols || !s->out_count)
-				return cb_fail(ctx, CBGPU_ERR_INVALID, "pipeline sink: output shape mismatch%s (%lld values)", "", depth);
+			if (!s->out || s->nout != xp->depth || s->nout > CBP_MAX_OUT || s->nout > s->out->ncols || !s->out_count)
+				return cb_fail(ctx, CBGPU_ERR_INVALID, "pipeline sink: output shape mismatch%s (%lld values)", "", xp->depth);
 			ds->nout = s->nout;
 			for (int c = 0; c < s->nout; c++)
 			{
@@ -276,16 +230,10 @@ cb_pipeline_to_dev(cbgpu_ctx *ctx, const CbPipeline *p, PipeDev *d)
 		d->stage_pc[ns++] = 0;
 		for (int i = 0; i < d->nops; i++)
 		{
-			int			c = d->ops[i].code;
+			const int	c = d->ops[i].code;
+			const XEffect e = xm_effect(d->ops[i], p->probes);
 
-			if (c == CBP_LOAD || c == CBP_CONST || c == CBP_DUP || c == XOP_MULCSUB)
-				dep++;
-			else if (c == CBP_FILTER || c == CBP_POP)
-				dep--;
-			else if (c == CBP_PROBE)
-				dep -= p->probes[d->ops[i].a].nkeys;
-			else if (c != CBP_NOT && c != CBP_I2F && c != CBP_F8ORD && c != CBP_END && c != XOP_FILTER_COL && c != XOP_PROBE_COLS)
-				dep--;
+			dep += e.pushes - e.pops;
 			if ((c == CBP_PROBE || c == XOP_PROBE_COLS) && dep == 0 && ns < CBP_MAX_STAGES && i + 1 < d->nops)
 				d->stage_pc[ns++] = i + 1;
 		}
@@ -796,10 +744,11 @@ extern "C" int
 cbgpu_pipeline_run(cbgpu_ctx *ctx, const CbPipeline *p)
 {
 	PipeDev    *dp = (PipeDev *) cb_scratch(ctx, 1, sizeof(PipeDev));	/* large: off the stack, per context (re-entrant) */
-	if (!dp)
+	XProg	   *xp = (XProg *) cb_scratch(ctx, 2, sizeof(XProg));
+	if (!dp || !xp)
 		return CBGPU_ERR_NOMEM;
 	PipeDev    &d = *dp;
-	int			rc = cb_pipeline_to_dev(ctx, p, &d);
+	int			rc = cb_pipeline_to_dev(ctx, p, &d, xp);
 	bool		handled = false;
 
 	if (rc)
@@ -824,7 +773,7 @@ cbgpu_pipeline_run(cbgpu_ctx *ctx, const CbPipeline *p)
 		multibatch = true;		/* ... nor of aggregate partitions */
 	if (!p->force_generic && !multibatch)
 	{
-		rc = cb_try_specialised(ctx, p, &d, &handled);
+		rc = cb_try_specialised(ctx, p, &d, xp, &handled);
 		if (rc)
 			return rc;
 	}

@@ -324,9 +324,11 @@ sink_store(void *col, int type, uint64_t pos, int64_t v)
 	}
 }
 
+struct XProg;					/* xmatch.h: the program's expression trees */
+
 void		cb_agg_touch(cbgpu_aggtable *t);
 int			cb_klog_begin(cbgpu_ctx *ctx, const char *name);
 void		cb_klog_end(cbgpu_ctx *ctx, int i);
-int			cb_pipeline_to_dev(cbgpu_ctx *ctx, const CbPipeline *p, PipeDev *d);
-int			cb_try_probe_chain(cbgpu_ctx *ctx, const CbPipeline *p, const PipeDev *d, bool *handled);
-int			cb_try_specialised(cbgpu_ctx *ctx, const CbPipeline *p, const PipeDev *d, bool *handled);
+int			cb_pipeline_to_dev(cbgpu_ctx *ctx, const CbPipeline *p, PipeDev *d, XProg *x);
+int			cb_try_probe_chain(cbgpu_ctx *ctx, const CbPipeline *p, const PipeDev *d, const XProg *x, bool *handled);
+int			cb_try_specialised(cbgpu_ctx *ctx, const CbPipeline *p, const PipeDev *d, const XProg *x, bool *handled);

@@ -1377,13 +1377,12 @@ k_pc_early_build(PcEarlyBuild B)
 	} while (0)
 
 int
-cb_try_probe_chain(cbgpu_ctx *ctx, const CbPipeline *p, const PipeDev *d, bool *handled)
+cb_try_probe_chain(cbgpu_ctx *ctx, const CbPipeline *p, const PipeDev *d, const XProg *xp, bool *handled)
 {
-	XProg	   *xp = (XProg *) cb_scratch(ctx, 2, sizeof(XProg));
 	PcParams   *Pp = (PcParams *) cb_scratch(ctx, 3, sizeof(PcParams));
-	if (!xp || !Pp)
+	if (!Pp)
 		return CBGPU_ERR_NOMEM;
-	XProg	   &x = *xp;
+	const XProg &x = *xp;
 	PcParams   &P = *Pp;
 	const CbpSink *s = &p->sink;
 	int			np = 0;
@@ -1397,45 +1396,28 @@ cb_try_probe_chain(cbgpu_ctx *ctx, const CbPipeline *p, const PipeDev *d, bool *
 		PC_REJECT(2);
 	if (s->kind == CBP_SINK_PARTITION && s->nsegs > 64)
 		PC_REJECT(2);
-	if (!xm_decompile(p, &x))
+	if (x.f8ord)
 		PC_REJECT(3);
 	memset(&P, 0, sizeof(P));
 	/* sections: quals (before the first probe only), then the probes in program order */
 	for (int i = 0; i < x.nsections; i++)
 	{
-		XSection   *sec = &x.sections[i];
+		const XSection *sec = &x.sections[i];
 
 		if (sec->kind == 0)
 		{
 			int			code, col;
-			int64_t		v, lo = INT32_MIN, hi = INT32_MAX;
+			int64_t		v, lo, hi;
 
 			if (np > 0)
 				PC_REJECT(4);	/* a qual behind a join: generic kernel */
 			if (!xm_is_cmp_const(&x, sec->node, &code, &col, &v) || p->cols[col].src != 0 || p->cols[col].nulls ||
 				(cb_type_w(p->cols[col].type) != 4 && cb_type_w(p->cols[col].type) != 1))
 				PC_REJECT(5);
-			if (cb_type_w(p->cols[col].type) == 1)
-			{
-				/* 1-byte columns hold unsigned values (cb_load_widen): clamp the range to them */
-				lo = 0;
-				hi = 255;
-			}
-			switch (code)
-			{
-				case CBP_EQ: lo = hi = v; break;
-				case CBP_LT: hi = v - 1; break;
-				case CBP_LE: hi = v; break;
-				case CBP_GT: lo = v + 1; break;
-				case CBP_GE: lo = v; break;
-				default: PC_REJECT(6);
-			}
-			if (lo > INT32_MAX || hi < INT32_MIN || lo > hi)
-				PC_REJECT(7);
-			if (hi > INT32_MAX)
-				hi = INT32_MAX;
-			if (lo < INT32_MIN)
-				lo = INT32_MIN;
+			const bool	byte = cb_type_w(p->cols[col].type) == 1;	/* unsigned values (cb_load_widen): [0, 255] */
+
+			if (!xm_qual_range(code, v, byte ? 0 : INT32_MIN, byte ? 255 : INT32_MAX, &lo, &hi))
+				PC_REJECT(6);
 			if (((uintptr_t) p->cols[col].data & 15) != 0)
 				PC_REJECT(100);		/* stage F reads the qual columns 16 bytes at a time */
 			{
@@ -1735,7 +1717,7 @@ cb_try_probe_chain(cbgpu_ctx *ctx, const CbPipeline *p, const PipeDev *d, bool *
 
 	if (P.nrows >= ctx->opt_pf_min_rows && np >= 1)	/* below ~16 M rows the fused kernel's fixed costs win */
 	{
-		PfParams   *Fp = (PfParams *) cb_scratch(ctx, 6, sizeof(PfParams));
+		PfParams   *Fp = (PfParams *) cb_scratch(ctx, 5, sizeof(PfParams));
 
 		if (!Fp)
 			return CBGPU_ERR_NOMEM;

@@ -501,12 +501,9 @@ col_plain(const CbPipeline *p, int c, int width)
 }
 
 static int
-try_small_agg(cbgpu_ctx *ctx, const CbPipeline *p, const PipeDev *d, bool *handled)
+try_small_agg(cbgpu_ctx *ctx, const CbPipeline *p, const PipeDev *d, const XProg *xp, bool *handled)
 {
-	XProg	   *xp = (XProg *) cb_scratch(ctx, 5, sizeof(XProg));
-	if (!xp)
-		return CBGPU_ERR_NOMEM;
-	XProg	   &x = *xp;
+	const XProg &x = *xp;
 	SmallAggParams P;
 	int			colB = -1,
 				colC = -1,
@@ -521,7 +518,7 @@ try_small_agg(cbgpu_ctx *ctx, const CbPipeline *p, const PipeDev *d, bool *handl
 	*handled = false;
 	if (s->kind != CBP_SINK_AGG || p->nprobes != 0 || p->drv_nsrc != 0 || s->nkeys > 2)
 		return CBGPU_OK;
-	if (!xm_decompile(p, &x) || x.depth < s->nkeys)
+	if (x.f8ord || x.depth < s->nkeys)
 		return CBGPU_OK;
 	memset(&P, 0, sizeof(P));
 	P.fspan = 0xFFFFFFFFu;		/* no qual: every value is inside the range */
@@ -532,27 +529,12 @@ try_small_agg(cbgpu_ctx *ctx, const CbPipeline *p, const PipeDev *d, bool *handl
 	{
 		int			code,
 					col;
-		int64_t		v;
+		int64_t		v,
+					lo,
+					hi;
 
 		if (x.sections[0].kind != 0 || !xm_is_cmp_const(&x, x.sections[0].node, &code, &col, &v) ||
-			!col_plain(p, col, 4) || v < INT32_MIN || v > INT32_MAX)
-			return CBGPU_OK;
-		/* fold the comparison into a closed int32 range (NE is not a range: generic kernel) */
-		int64_t		lo = INT32_MIN,
-					hi = INT32_MAX;
-
-		switch (code)
-		{
-			case CBP_EQ: lo = hi = v; break;
-			case CBP_LT: hi = v - 1; break;
-			case CBP_LE: hi = v; break;
-			case CBP_GT: lo = v + 1; break;
-			case CBP_GE: lo = v; break;
-			default: return CBGPU_OK;
-		}
-		if (lo > hi)
-			lo = hi = (int64_t) INT32_MAX + 1;	/* empty range: handled below */
-		if (lo > INT32_MAX || hi < INT32_MIN)
+			!col_plain(p, col, 4) || v < INT32_MIN || v > INT32_MAX || !xm_qual_range(code, v, INT32_MIN, INT32_MAX, &lo, &hi))
 			return CBGPU_OK;
 		P.fcol = (const int32_t *) p->cols[col].data;
 		P.flo = (int32_t) lo;
@@ -804,11 +786,11 @@ try_small_agg(cbgpu_ctx *ctx, const CbPipeline *p, const PipeDev *d, bool *handl
 }
 
 int
-cb_try_specialised(cbgpu_ctx *ctx, const CbPipeline *p, const PipeDev *d, bool *handled)
+cb_try_specialised(cbgpu_ctx *ctx, const CbPipeline *p, const PipeDev *d, const XProg *x, bool *handled)
 {
-	int			rc = try_small_agg(ctx, p, d, handled);
+	int			rc = try_small_agg(ctx, p, d, x, handled);
 
 	if (rc != CBGPU_OK || *handled)
 		return rc;
-	return cb_try_probe_chain(ctx, p, d, handled);
+	return cb_try_probe_chain(ctx, p, d, x, handled);
 }

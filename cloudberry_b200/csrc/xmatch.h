@@ -1,13 +1,11 @@
 /*
- * xmatch.h - host-side reconstruction of expression trees from a pipeline's postfix program, used
- * by the pattern matchers that route a descriptor to a hand-fused kernel (the role the reference's
- * ExecReadyInterpretedExpr / EEOP fast-path selection plays for common expression shapes,
- * backend/executor/execExprInterp.c:260-330).
+ * xmatch.h - the host's one reading of a postfix program (a pipeline's or a join filter's): what each op does to the value
+ * stack, the walk that checks a program and rebuilds its expression trees, and the helpers the pattern matchers use to
+ * route a descriptor to a hand-fused kernel (the role the reference's ExecReadyInterpretedExpr / EEOP fast-path selection
+ * plays for common expression shapes, backend/executor/execExprInterp.c:260-330).
  */
 #pragma once
-#include "common.cuh"
-
-#define XM_MAXNODES 320
+#include "pipeline.cuh"
 
 struct XNode
 {
@@ -27,79 +25,119 @@ struct XSection
 
 struct XProg
 {
-	XNode		nodes[XM_MAXNODES];
+	XNode		nodes[CBP_MAX_OPS];	/* an op makes at most one node */
 	int			n;
 	XSection	sections[CBP_MAX_OPS];
 	int			nsections;
 	int			stack[CBP_STACK];	/* node ids left on the stack at END: keys then args / outputs    */
 	int			depth;
+	bool		f8ord;			/* the program holds an F8ORD: float arithmetic stays with the generic kernel */
 };
 
-static inline bool
-xm_decompile(const CbPipeline *p, XProg *x)
+/* the values an op pops and pushes, internal fused ops (pipeline.cuh) included; PROBE pops its probe's keys */
+struct XEffect
+{
+	int			pops,
+				pushes;
+};
+
+static inline XEffect
+xm_effect(const CbpOp &op, const CbpProbe *probes)
+{
+	switch (op.code)
+	{
+		case CBP_LOAD: case CBP_CONST: case CBP_DUP: case XOP_MULCSUB:
+			return {0, 1};
+		case CBP_NOT: case CBP_I2F: case CBP_F8ORD:
+			return {1, 1};
+		case CBP_FILTER: case CBP_POP:
+			return {1, 0};
+		case CBP_PROBE:
+			return {probes[op.a].nkeys, 0};
+		case CBP_END: case XOP_FILTER_COL: case XOP_PROBE_COLS:
+			return {0, 0};
+		default:				/* binary operators */
+			return {2, 1};
+	}
+}
+
+/* opcodes as bits of XAllow.ops */
+#define XM_OP(c) (1u << (c))
+#define XM_PIPELINE_OPS (XM_OP(CBP_F8ORD + 1) - 1)	/* every CbpOpCode (F8ORD is the last) */
+#define XM_SCALAR_OPS (XM_PIPELINE_OPS & ~(XM_OP(CBP_FILTER) | XM_OP(CBP_PROBE) | XM_OP(CBP_END)))
+
+/* what a caller lets a program hold, and how it reports a refusal */
+struct XAllow
+{
+	const char *what;			/* "pipeline" / "join filter": the subject of the messages           */
+	uint32_t	ops;			/* XM_OP(code) set: the opcodes allowed (END only as the last op)     */
+	const CbpProbe *probes;		/* PROBE a takes probes[a], a < nprobes                               */
+	int			nprobes;
+	int			too_deep;		/* the code of a stack deeper than CBP_STACK                          */
+};
+
+/* Checks a program of 1 .. CBP_MAX_OPS ops over `ncols` columns op by op and builds its expression trees in *x: FILTER and
+ * PROBE close a section, what is left on the stack at the end is x->stack[0 .. x->depth).  CBGPU_ERR_INVALID for a bad LOAD
+ * column or DUP index, a bad PROBE, a stack underflow, an END before the last op and an opcode the caller does not allow;
+ * allow.too_deep for a stack deeper than CBP_STACK.  The caller checks the final state. */
+static inline int
+xm_walk(cbgpu_ctx *ctx, const XAllow &allow, int ncols, const CbpOp *ops, int nops, XProg *x)
 {
 	x->n = 0;
 	x->nsections = 0;
 	x->depth = 0;
-	for (int i = 0; i < p->nops; i++)
+	x->f8ord = false;
+	for (int i = 0; i < nops; i++)
 	{
-		const CbpOp *op = &p->ops[i];
+		const CbpOp *op = &ops[i];
 
+		if (op->code < 0 || op->code >= 32 || !(allow.ops & XM_OP(op->code)))
+			return cb_fail(ctx, CBGPU_ERR_INVALID, "%s op %lld: opcode not supported", allow.what, i);
+		if (op->code == CBP_LOAD && (op->a < 0 || op->a >= ncols))
+			return cb_fail(ctx, CBGPU_ERR_INVALID, "%s op %lld: LOAD of a missing column", allow.what, i);
+		if (op->code == CBP_DUP && (op->a < 0 || op->a >= x->depth))
+			return cb_fail(ctx, CBGPU_ERR_INVALID, "%s op %lld: DUP out of range", allow.what, i);
+		if (op->code == CBP_PROBE && (op->a < 0 || op->a >= allow.nprobes || allow.probes[op->a].nkeys < 0 ||
+									  allow.probes[op->a].nkeys > CBP_MAX_KEYS))
+			return cb_fail(ctx, CBGPU_ERR_INVALID, "%s op %lld: bad PROBE", allow.what, i);
+		if (op->code == CBP_END && i != nops - 1)
+			return cb_fail(ctx, CBGPU_ERR_INVALID, "%s op %lld: END before the last op", allow.what, i);
+		const XEffect e = xm_effect(*op, allow.probes);
+		const int	base = x->depth - e.pops;	/* where the op's values start on the stack */
+
+		if (base < 0)
+			return cb_fail(ctx, CBGPU_ERR_INVALID, "%s op %lld: stack underflow", allow.what, i);
+		if (base + e.pushes > CBP_STACK)
+			return cb_fail(ctx, allow.too_deep, "%s op %lld: stack deeper than CBP_STACK", allow.what, i);
 		switch (op->code)
 		{
-			case CBP_LOAD:
-			case CBP_CONST:
-				if (x->n >= XM_MAXNODES)
-					return false;
-				x->nodes[x->n] = {op->code, op->a, op->imm, -1, -1};
-				x->stack[x->depth++] = x->n++;
-				break;
 			case CBP_DUP:
-				x->stack[x->depth] = x->stack[op->a];
-				x->depth++;
-				break;
-			case CBP_POP:
-				x->depth--;
-				break;
-			case CBP_F8ORD:
-				return false;		/* float arithmetic stays with the generic kernel */
-			case CBP_NOT:
-			case CBP_I2F:
-				if (x->n >= XM_MAXNODES)
-					return false;
-				x->nodes[x->n] = {op->code, op->a, 0, x->stack[x->depth - 1], -1};
-				x->stack[x->depth - 1] = x->n++;
+				x->stack[base] = x->stack[op->a];
 				break;
 			case CBP_FILTER:
-				x->depth--;
-				x->sections[x->nsections].kind = 0;
-				x->sections[x->nsections].node = x->stack[x->depth];
-				x->nsections++;
+				x->sections[x->nsections++] = {0, x->stack[base], -1, {}};
 				break;
 			case CBP_PROBE:
 				{
-					int			nk = p->probes[op->a].nkeys;
+					XSection   *s = &x->sections[x->nsections++];
 
-					x->depth -= nk;
-					x->sections[x->nsections].kind = 1;
-					x->sections[x->nsections].probe = op->a;
-					for (int k = 0; k < nk; k++)
-						x->sections[x->nsections].keys[k] = x->stack[x->depth + k];
-					x->nsections++;
+					*s = {1, -1, op->a, {}};
+					for (int k = 0; k < e.pops; k++)
+						s->keys[k] = x->stack[base + k];
 					break;
 				}
+			case CBP_POP:
 			case CBP_END:
 				break;
-			default:			/* binary operators */
-				if (x->n >= XM_MAXNODES)
-					return false;
-				x->nodes[x->n] = {op->code, op->a, 0, x->stack[x->depth - 2], x->stack[x->depth - 1]};
-				x->depth--;
-				x->stack[x->depth - 1] = x->n++;
+			default:			/* LOAD, CONST and the operators: one node over the values they pop */
+				x->nodes[x->n] = {op->code, op->a, op->imm, e.pops > 0 ? x->stack[base] : -1, e.pops > 1 ? x->stack[base + 1] : -1};
+				x->stack[base] = x->n++;
+				x->f8ord |= op->code == CBP_F8ORD;
 				break;
 		}
+		x->depth = base + e.pushes;
 	}
-	return true;
+	return CBGPU_OK;
 }
 
 static inline bool
@@ -158,4 +196,29 @@ xm_is_cmp_const(const XProg *x, int node, int *code, int *col, int64_t *v)
 		return false;
 	*code = c;
 	return xm_is_load(x, x->nodes[node].l, col) && xm_is_const(x, x->nodes[node].r, v);
+}
+
+/* The rows `col CMP v` keeps, as a closed range [*lo, *hi] inside int32, over a column whose values lie in [dlo, dhi]
+ * (inside int32): EQ keeps [v, v], the other compares bound one end of the domain.  False for NE (not a range) and for an
+ * empty range. */
+static inline bool
+xm_qual_range(int code, int64_t v, int64_t dlo, int64_t dhi, int64_t *lo, int64_t *hi)
+{
+	int64_t		l = dlo,
+				h = dhi;
+
+	switch (code)
+	{
+		case CBP_EQ: l = h = v; break;
+		case CBP_LT: if (v == INT64_MIN) return false; h = v - 1; break;
+		case CBP_LE: h = v; break;
+		case CBP_GT: if (v == INT64_MAX) return false; l = v + 1; break;
+		case CBP_GE: l = v; break;
+		default: return false;
+	}
+	if (l > h || l > INT32_MAX || h < INT32_MIN)
+		return false;
+	*lo = l < INT32_MIN ? INT32_MIN : l;
+	*hi = h > INT32_MAX ? INT32_MAX : h;
+	return true;
 }
