@@ -52,7 +52,7 @@ class CbgpuJoinFilter(C.Structure):
 # CbpOpCode
 (CBP_END, CBP_LOAD, CBP_CONST, CBP_ADD, CBP_SUB, CBP_MUL, CBP_FADD, CBP_FSUB, CBP_FMUL, CBP_I2F, CBP_EQ, CBP_NE, CBP_LT, CBP_LE,
  CBP_GT, CBP_GE, CBP_FEQ, CBP_FNE, CBP_FLT, CBP_FLE, CBP_FGT, CBP_FGE, CBP_AND, CBP_OR, CBP_NOT, CBP_FILTER, CBP_PROBE, CBP_DUP,
- CBP_POP, CBP_F8ORD) = range(30)
+ CBP_POP, CBP_F8ORD, CBP_INSET) = range(31)
 
 
 def join_filter(cols, ops):
@@ -194,11 +194,41 @@ def aocs_segfile_path(basepath, segno, filenum):
 class DeviceDict:
     """dictionary of a bpchar(n) / varchar / text column, built on the device from the column's files (cbgpu_dict)"""
 
-    def __init__(self, ctx, max_entries=4096, arena_bytes=1 << 20, bpchar=True):
+    def __init__(self, ctx, max_entries=4096, arena_bytes=1 << 20, bpchar=True, handle=None):
         self.ctx = ctx
+        if handle is None:
+            handle = C.c_void_p()
+            ctx.check(ctx.L.cbgpu_dict_create(ctx.h, max_entries, arena_bytes, 1 if bpchar else 0, C.byref(handle)))
+        self.h = handle
+
+    @classmethod
+    def from_texts(cls, ctx, texts, bpchar=False):
+        """a finalized dictionary whose code c is texts[c] (distinct, in byte order; bpchar: without trailing blanks)"""
+        bs = [t if isinstance(t, bytes) else t.encode() for t in texts]
+        n = len(bs)
+        arr = (C.c_char_p * max(n, 1))(*bs)
+        lens = (C.c_int32 * max(n, 1))(*[len(b) for b in bs])
         h = C.c_void_p()
-        ctx.check(ctx.L.cbgpu_dict_create(ctx.h, max_entries, arena_bytes, 1 if bpchar else 0, C.byref(h)))
-        self.h = h
+        ctx.check(ctx.L.cbgpu_dict_from_texts(ctx.h, n, arr, lens, 1 if bpchar else 0, C.byref(h)))
+        return cls(ctx, handle=h)
+
+    def nentries(self):
+        return int(self.ctx.L.cbgpu_dict_nentries(self.h))
+
+    def match_like(self, pattern, bpchar_len=0):
+        """LIKE of every entry on the device (k_dict_like): a list of booleans by code"""
+        p = pattern if isinstance(pattern, bytes) else pattern.encode()
+        n = self.nentries()
+        nw = (n + 31) // 32
+        dev = C.c_void_p()
+        self.ctx.check(self.ctx.L.cbgpu_dev_alloc(self.ctx.h, 4 * max(nw, 1), C.byref(dev)))
+        try:
+            self.ctx.check(self.ctx.L.cbgpu_dict_match_like(self.ctx.h, self.h, p, len(p), bpchar_len, dev))
+            words = np.zeros(max(nw, 1), dtype=np.uint32)
+            self.ctx.check(self.ctx.L.cbgpu_read_u32(self.ctx.h, dev, nw, words.ctypes.data))
+        finally:
+            self.ctx.L.cbgpu_dev_free(self.ctx.h, dev)
+        return [bool((words[c >> 5] >> (c & 31)) & 1) for c in range(n)]
 
     def collect(self, file_bytes, checksum, compresstype=0, typalign=4):
         buf = np.frombuffer(file_bytes, dtype=np.uint8)
@@ -350,6 +380,11 @@ def gpu():
             "cbgpu_dict_finalize": (C.c_int, [vp, C.POINTER(i32)]),
             "cbgpu_dict_entry": (C.c_int, [vp, i32, C.POINTER(C.c_char_p), C.POINTER(i32)]),
             "cbgpu_dict_lookup": (i32, [vp, C.c_char_p, i32]),
+            "cbgpu_dict_nentries": (i32, [vp]),
+            "cbgpu_dict_is_bpchar": (i32, [vp]),
+            "cbgpu_dict_from_texts": (C.c_int, [vp, i32, C.POINTER(C.c_char_p), C.POINTER(i32), i32, C.POINTER(vp)]),
+            "cbgpu_dict_match_like": (C.c_int, [vp, vp, C.c_char_p, i32, i32, vp]),
+            "cbgpu_rel_set_dict": (C.c_int, [vp, i32, vp, i32]),
             "cbgpu_aocs_decode_dict_column": (C.c_int, [vp, vp, i64, i32, i32, i32, vp, vp, i32, i64, C.POINTER(i64)]),
             "cbgpu_aocs_apply_visimap": (C.c_int, [vp, vp, i64, i32, vp, i32, vp, i64, C.POINTER(i64)]),
             "cbgpu_rel_set_dict_hash": (C.c_int, [vp, i32, vp, i32]),
@@ -743,6 +778,11 @@ class DeviceRelation:
     def set_dict_hash(self, col, hashes):
         dh = np.ascontiguousarray(hashes, dtype=np.uint32)
         self.ctx.check(self.ctx.L.cbgpu_rel_set_dict_hash(self.h, col, dh.ctypes.data, len(dh)))
+
+    def set_dict(self, col, dictionary, bpchar_len=0):
+        """link column `col` to its DeviceDict (borrowed: keep the dictionary alive) so LIKE and IN lists can run over it;
+        bpchar_len = n of a character(n) column, 0 for varchar / text"""
+        self.ctx.check(self.ctx.L.cbgpu_rel_set_dict(self.h, col, dictionary.h, bpchar_len))
 
     def read_column(self, col, lo=0, hi=None):
         hi = self.rows() if hi is None else hi

@@ -41,6 +41,7 @@
  */
 #include "common.cuh"
 #include "inflate.cuh"
+#include "like_match.cuh"
 #include "zstd_dec.cuh"
 
 #include <stdlib.h>
@@ -740,7 +741,7 @@ k_aocs_unzstd(uint8_t *raw, const AocsDir *dir, int nblocks, int *status, int *a
  * assigns codes; LOOKUP finds the tag again and now also compares the bytes, so two different strings with one 64-bit
  * hash are reported (CBGPU_ERR_UNSUPPORTED) instead of sharing a code.
  * --------------------------------------------------------------------------------------------- */
-__device__ __forceinline__ unsigned long long
+__host__ __device__ __forceinline__ unsigned long long
 dict_hash64(const uint8_t *p, int n)
 {
 	unsigned long long h = 0xcbf29ce484222325ull;	/* FNV-1a, then a finaliser */
@@ -1362,6 +1363,7 @@ struct cbgpu_dict
 	uint8_t    *d_arena;
 	unsigned long long *d_cursor;
 	uint32_t   *d_hashes;		/* per code, after finalize                                           */
+	uint2	   *d_offlen;		/* per code, after finalize: (offset, length) of its bytes in d_arena */
 	uint32_t	nslots;
 	uint32_t	arena_cap;
 	int32_t		max_entries;
@@ -1573,6 +1575,8 @@ cbgpu_dict_free(cbgpu_dict *d)
 		cudaFreeAsync(d->d_cursor, d->ctx->stream);
 	if (d->d_hashes)
 		cudaFreeAsync(d->d_hashes, d->ctx->stream);
+	if (d->d_offlen)
+		cudaFreeAsync(d->d_offlen, d->ctx->stream);
 	free(d->texts);
 	free(d->off);
 	free(d->len);
@@ -1619,6 +1623,11 @@ cbgpu_aocs_decode_dict_column(cbgpu_ctx *ctx, const void *file_bytes, int64_t nb
 									 ctx->stream));
 		rel->dict_n[col] = dict->n;
 	}
+	/* the declared n of a character(n) column is the loader's to give (cbgpu_rel_set_dict); until it does, -1 = unknown, and a
+	 * LIKE over the column is refused rather than matched without its padding */
+	if (rel->dict[col] != dict)
+		rel->dict_bpchar_len[col] = dict->bpchar ? -1 : 0;
+	rel->dict[col] = dict;
 	return CBGPU_OK;
 }
 
@@ -1638,6 +1647,35 @@ dict_slot_cmp(const void *a, const void *b)
 	return x->len < y->len ? -1 : x->len > y->len;
 }
 
+/* The last step of building a dictionary whose entries are in code order on the host (texts, off[], len[], and the slot
+ * table with the codes assigned): the per-code hashes, the slot table and the per-code (offset, length) pairs k_dict_like
+ * reads go to the device. */
+static int
+dict_publish(cbgpu_dict *d, CbCallMem *mem, const DictSlot *slots, int32_t n)
+{
+	cbgpu_ctx  *ctx = d->ctx;
+	uint32_t   *hashes = mem->keep((uint32_t *) malloc(sizeof(uint32_t) * (size_t) (n ? n : 1)));
+	uint2	   *offlen = mem->keep((uint2 *) malloc(sizeof(uint2) * (size_t) (n ? n : 1)));
+
+	if (!hashes || !offlen)
+		return CBGPU_ERR_NOMEM;
+	for (int32_t c = 0; c < n; c++)
+	{
+		/* hashbpchar over the blank-trimmed bytes == hashtext over the same bytes: both hash_any (utils/adt/varchar.c:981-1010) */
+		hashes[c] = pg_hash_bytes_host((const unsigned char *) d->texts + d->off[c], (int) d->len[c]);
+		offlen[c] = make_uint2(d->off[c], d->len[c]);
+	}
+	CB_CUDA(ctx, mem->copy_in(d->d_slots, slots, sizeof(DictSlot) * (size_t) d->nslots));
+	CB_CUDA(ctx, cudaMallocAsync(&d->d_hashes, sizeof(uint32_t) * (size_t) (n ? n : 1), ctx->stream));
+	CB_CUDA(ctx, mem->copy_in(d->d_hashes, hashes, sizeof(uint32_t) * (size_t) n));
+	CB_CUDA(ctx, cudaMallocAsync(&d->d_offlen, sizeof(uint2) * (size_t) (n ? n : 1), ctx->stream));
+	CB_CUDA(ctx, mem->copy_in(d->d_offlen, offlen, sizeof(uint2) * (size_t) n));
+	CB_CUDA(ctx, mem->sync());
+	d->n = n;
+	d->finalized = 1;
+	return CBGPU_OK;
+}
+
 extern "C" int
 cbgpu_dict_finalize(cbgpu_dict *d, int32_t *nentries)
 {
@@ -1645,7 +1683,6 @@ cbgpu_dict_finalize(cbgpu_dict *d, int32_t *nentries)
 	CbCallMem	mem(ctx);
 	DictSlot   *slots;
 	unsigned long long cur[2];
-	uint32_t   *hashes;
 	int32_t		n = 0;
 	int			rc;
 
@@ -1668,8 +1705,7 @@ cbgpu_dict_finalize(cbgpu_dict *d, int32_t *nentries)
 	d->sorted = (int32_t *) malloc(sizeof(int32_t) * (size_t) (cur[1] ? cur[1] : 1));
 	d->off = (uint32_t *) malloc(sizeof(uint32_t) * (size_t) (cur[1] ? cur[1] : 1));
 	d->len = (uint32_t *) malloc(sizeof(uint32_t) * (size_t) (cur[1] ? cur[1] : 1));
-	hashes = mem.keep((uint32_t *) malloc(sizeof(uint32_t) * (size_t) (cur[1] ? cur[1] : 1)));
-	if (!slots || !d->texts || !d->sorted || !d->off || !d->len || !hashes)
+	if (!slots || !d->texts || !d->sorted || !d->off || !d->len)
 		return CBGPU_ERR_NOMEM;
 	CB_CUDA(ctx, cudaMemcpyAsync(slots, d->d_slots, sizeof(DictSlot) * (size_t) d->nslots, cudaMemcpyDeviceToHost, ctx->stream));
 	CB_CUDA(ctx, cudaMemcpyAsync(d->texts, d->d_arena, (size_t) cur[0], cudaMemcpyDeviceToHost, ctx->stream));
@@ -1689,18 +1725,11 @@ cbgpu_dict_finalize(cbgpu_dict *d, int32_t *nentries)
 		sl->code = c;
 		d->off[c] = sl->off;
 		d->len[c] = sl->len;
-		/* hashbpchar over the blank-trimmed bytes == hashtext over the same bytes: both hash_any (utils/adt/varchar.c:981-1010) */
-		hashes[c] = pg_hash_bytes_host((const unsigned char *) d->texts + sl->off, (int) sl->len);
 	}
-	CB_CUDA(ctx, mem.copy_in(d->d_slots, slots, sizeof(DictSlot) * (size_t) d->nslots));
-	CB_CUDA(ctx, cudaMallocAsync(&d->d_hashes, sizeof(uint32_t) * (size_t) (n ? n : 1), ctx->stream));
-	CB_CUDA(ctx, mem.copy_in(d->d_hashes, hashes, sizeof(uint32_t) * (size_t) n));
-	CB_CUDA(ctx, mem.sync());
-	d->n = n;
-	d->finalized = 1;
-	if (nentries)
+	rc = dict_publish(d, &mem, slots, n);
+	if (rc == CBGPU_OK && nentries)
 		*nentries = n;
-	return CBGPU_OK;
+	return rc;
 }
 
 extern "C" int
@@ -1741,6 +1770,174 @@ cbgpu_dict_lookup(const cbgpu_dict *d, const char *text, int32_t len)
 			hi = mid - 1;
 	}
 	return -1;
+}
+
+extern "C" int32_t
+cbgpu_dict_nentries(const cbgpu_dict *d)
+{
+	return d && d->finalized ? d->n : 0;
+}
+
+extern "C" int32_t
+cbgpu_dict_is_bpchar(const cbgpu_dict *d)
+{
+	return d && d->bpchar;
+}
+
+static int
+dict_text_cmp(const char *a, int32_t la, const char *b, int32_t lb)
+{
+	const int	c = memcmp(a, b, (size_t) (la < lb ? la : lb));
+
+	return c ? c : la < lb ? -1 : la > lb;
+}
+
+extern "C" int
+cbgpu_dict_from_texts(cbgpu_ctx *ctx, int32_t n, const char *const *texts, const int32_t *lens, int32_t bpchar, cbgpu_dict **out)
+{
+	int64_t		arena = 0;
+	cbgpu_dict *raw = NULL;
+	unsigned long long cur[2];
+	int			rc;
+
+	*out = NULL;
+	if (n < 0 || (n > 0 && (!texts || !lens)))
+		return cb_fail(ctx, CBGPU_ERR_INVALID, "cbgpu_dict_from_texts: %s%lld strings", "", n);
+	for (int32_t c = 0; c < n; c++)
+	{
+		if (lens[c] < 0 || (lens[c] > 0 && !texts[c]))
+			return cb_fail(ctx, CBGPU_ERR_INVALID, "cbgpu_dict_from_texts: string %s%lld is malformed", "", c);
+		if (bpchar && lens[c] > 0 && texts[c][lens[c] - 1] == ' ')
+			return cb_fail(ctx, CBGPU_ERR_INVALID, "cbgpu_dict_from_texts: string %s%lld of a bpchar dictionary has trailing blanks", "", c);
+		if (c > 0 && dict_text_cmp(texts[c - 1], lens[c - 1], texts[c], lens[c]) >= 0)
+			return cb_fail(ctx, CBGPU_ERR_INVALID, "cbgpu_dict_from_texts: string %s%lld is not above the one before it in byte order", "", c);
+		arena += (lens[c] + 3) & ~3;
+		if (arena > 0xFFFFFFF0ll)
+			return cb_fail(ctx, CBGPU_ERR_INVALID, "cbgpu_dict_from_texts: %s%lld strings exceed the arena's 32-bit offsets", "", n);
+	}
+	rc = cbgpu_dict_create(ctx, n > 0 ? n : 1, arena < 16 ? 16 : arena, bpchar, &raw);
+	if (rc)
+		return rc;
+	CbOwned<cbgpu_dict> d(raw, cbgpu_dict_free);
+	CbCallMem	mem(ctx);
+	DictSlot   *slots = mem.keep((DictSlot *) calloc(d->nslots, sizeof(DictSlot)));
+	uint32_t	pos = 0;
+
+	d->texts = (char *) malloc((size_t) arena + 16);
+	d->sorted = (int32_t *) malloc(sizeof(int32_t) * (size_t) (n ? n : 1));
+	d->off = (uint32_t *) malloc(sizeof(uint32_t) * (size_t) (n ? n : 1));
+	d->len = (uint32_t *) malloc(sizeof(uint32_t) * (size_t) (n ? n : 1));
+	if (!slots || !d->texts || !d->sorted || !d->off || !d->len)
+		return CBGPU_ERR_NOMEM;
+	/* the slot table the collect pass would have built: the same tags and probe sequence, so that
+	 * cbgpu_aocs_decode_dict_column finds these strings as it finds collected ones */
+	for (int32_t c = 0; c < n; c++)
+	{
+		const unsigned long long tag = dict_hash64((const uint8_t *) texts[c], lens[c]);
+		uint32_t	i = (uint32_t) tag & (d->nslots - 1);
+
+		while (slots[i].tag)
+			i = (i + 1) & (d->nslots - 1);
+		slots[i] = {tag, pos, (uint32_t) lens[c], c, 0};
+		if (lens[c] > 0)
+			memcpy(d->texts + pos, texts[c], (size_t) lens[c]);
+		d->sorted[c] = (int32_t) i;
+		d->off[c] = pos;
+		d->len[c] = (uint32_t) lens[c];
+		pos += (uint32_t) ((lens[c] + 3) & ~3);
+	}
+	cur[0] = pos;
+	cur[1] = (unsigned long long) n;
+	CB_CUDA(ctx, mem.copy_in(d->d_arena, d->texts, pos));
+	CB_CUDA(ctx, mem.copy_in(d->d_cursor, cur, sizeof(cur)));
+	rc = dict_publish(d.get(), &mem, slots, n);
+	if (rc)
+		return rc;
+	*out = d.release();
+	return CBGPU_OK;
+}
+
+/* ---- LIKE over a dictionary: one match per distinct string, a bitmap over the codes ---- */
+#define LIKE_MAX_PATTERN 2048
+#define LIKE_THREADS 256
+
+struct DictLikeParams
+{
+	const uint8_t *arena;
+	const uint2 *offlen;
+	uint32_t   *bits;			/* ceil(n / 32) words, bit c of word c / 32 = code c matches          */
+	int32_t		n;
+	int32_t		bpchar_len;		/* character(n): n, the entries are matched blank-padded to n characters; 0 otherwise */
+	int32_t		plen;
+	uint8_t		pat[LIKE_MAX_PATTERN];
+};
+
+/* One thread per entry; every lane of a warp steps through the loop together, so the warp's 32 results are one ballot and
+ * one word store.  The pattern is read by every thread at its own position: it is staged in shared memory. */
+__global__ void __launch_bounds__(LIKE_THREADS)
+k_dict_like(const __grid_constant__ DictLikeParams P)
+{
+	__shared__ uint8_t pat[LIKE_MAX_PATTERN];
+
+	for (int i = threadIdx.x; i < P.plen; i += blockDim.x)
+		pat[i] = P.pat[i];
+	__syncthreads();
+	for (int64_t base = (int64_t) blockIdx.x * blockDim.x; base < P.n; base += (int64_t) gridDim.x * blockDim.x)
+	{
+		const int64_t c = base + threadIdx.x;
+		bool		m = false;
+
+		if (c < P.n)
+		{
+			const uint2 ol = P.offlen[c];
+			const uint8_t *t = P.arena + ol.x;
+			int			pad = P.bpchar_len > 0 ? P.bpchar_len - like_utf8_chars(t, (int) ol.y) : 0;
+
+			m = like_match(t, (int) ol.y, pad > 0 ? pad : 0, pat, P.plen);
+		}
+		const uint32_t w = __ballot_sync(0xffffffffu, m);
+
+		if ((threadIdx.x & 31) == 0 && c < P.n)
+			P.bits[c >> 5] = w;
+	}
+}
+
+extern "C" int
+cbgpu_dict_match_like(cbgpu_ctx *ctx, const cbgpu_dict *dict, const char *pattern, int32_t len, int32_t bpchar_len, uint32_t *bits_dev)
+{
+	DictLikeParams *P;
+	int64_t		blocks;
+
+	if (!dict || !dict->finalized || len < 0 || (len > 0 && !pattern) || (dict->n > 0 && !bits_dev))
+		return cb_fail(ctx, CBGPU_ERR_INVALID, "cbgpu_dict_match_like: bad argument%s (%lld)", "", len);
+	/* a bpchar dictionary holds its strings blank-trimmed: matching them needs the column's n, and only it has one */
+	if (dict->bpchar ? bpchar_len < 1 : bpchar_len != 0)
+		return cb_fail(ctx, CBGPU_ERR_INVALID, "cbgpu_dict_match_like: %sbpchar_len %lld does not fit the dictionary (character(n) needs n >= 1, "
+					   "varchar / text 0)", "", bpchar_len);
+	if (like_pattern_check((const uint8_t *) pattern, len))
+		return cb_fail(ctx, CBGPU_ERR_INVALID, "LIKE pattern must not end with escape character%s", "", 0);
+	if (len > LIKE_MAX_PATTERN)
+		return cb_fail(ctx, CBGPU_ERR_UNSUPPORTED, "LIKE pattern of %s%lld bytes is longer than the GPU path takes", "", len);
+	if (dict->n == 0)
+		return CBGPU_OK;
+	P = (DictLikeParams *) cb_scratch(ctx, 0, sizeof(DictLikeParams));
+	if (!P)
+		return CBGPU_ERR_NOMEM;
+	P->arena = dict->d_arena;
+	P->offlen = dict->d_offlen;
+	P->bits = bits_dev;
+	P->n = dict->n;
+	P->bpchar_len = bpchar_len;
+	P->plen = len;
+	if (len > 0)
+		memcpy(P->pat, pattern, (size_t) len);
+	blocks = ((int64_t) dict->n + LIKE_THREADS - 1) / LIKE_THREADS;
+	if (blocks > (int64_t) ctx->sm_count * 16)
+		blocks = (int64_t) ctx->sm_count * 16;
+	CB_CUDA(ctx, cudaSetDevice(ctx->device));
+	k_dict_like<<<(int) blocks, LIKE_THREADS, 0, ctx->stream>>>(*P);
+	CB_LAUNCHED(ctx, "k_dict_like");
+	return CBGPU_OK;
 }
 
 /* ---------------------------------------------------------------------------------------------

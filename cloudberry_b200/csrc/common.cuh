@@ -112,6 +112,8 @@ struct cbgpu_rel
 	uint8_t	   *visimap;
 	bool		owns[CB_MAX_COLS_REL];
 	void	   *slab;			/* small relations: the one allocation all columns live in (owns[] = false) */
+	const cbgpu_dict *dict[CB_MAX_COLS_REL];	/* borrowed (cbgpu_rel_set_dict), NULL: none       */
+	int32_t		dict_bpchar_len[CB_MAX_COLS_REL];
 };
 
 /* agg table, device view (struct of arrays; open addressing, linear probing) */

@@ -960,5 +960,30 @@ cbgpu_rel_share_dict_hash(cbgpu_rel *dst, int32_t dcol, const cbgpu_rel *src, in
 	dst->dict_hash[dcol] = src->dict_hash[scol];
 	/* negative count: borrowed, not freed with dst (the source may itself be a borrower) */
 	dst->dict_n[dcol] = src->dict_n[scol] > 0 ? -src->dict_n[scol] : (src->dict_n[scol] < 0 ? src->dict_n[scol] : -1);
+	dst->dict[dcol] = src->dict[scol];
+	dst->dict_bpchar_len[dcol] = src->dict_bpchar_len[scol];
 	return CBGPU_OK;
+}
+
+extern "C" int
+cbgpu_rel_set_dict(cbgpu_rel *rel, int32_t col, const cbgpu_dict *dict, int32_t bpchar_len)
+{
+	if (col < 0 || col >= rel->ncols || (rel->types[col] != CB_DICT8 && rel->types[col] != CB_DICT32) || !dict)
+		return cb_fail(rel->ctx, CBGPU_ERR_INVALID, "cbgpu_rel_set_dict: bad argument%s %lld", "", col);
+	if (cbgpu_dict_is_bpchar(dict) ? bpchar_len < 1 : bpchar_len != 0)
+		return cb_fail(rel->ctx, CBGPU_ERR_INVALID, "cbgpu_rel_set_dict: %sbpchar_len %lld does not fit the dictionary (character(n) "
+					   "needs n >= 1, varchar / text 0)", "", bpchar_len);
+	rel->dict[col] = dict;
+	rel->dict_bpchar_len[col] = bpchar_len;
+	return CBGPU_OK;
+}
+
+extern "C" const cbgpu_dict *
+cbgpu_rel_dict(const cbgpu_rel *rel, int32_t col, int32_t *bpchar_len)
+{
+	if (col < 0 || col >= rel->ncols)
+		return NULL;
+	if (bpchar_len)
+		*bpchar_len = rel->dict_bpchar_len[col];
+	return rel->dict[col];
 }

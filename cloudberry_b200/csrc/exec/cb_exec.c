@@ -26,6 +26,7 @@
 #include <string.h>
 
 #include "../../../include/cb_exec.h"
+#include "../like_match.cuh"		/* like_pattern_check: a malformed pattern is refused while the plan translates */
 
 /* ------------------------------------------------------------------------------------------
  * errors
@@ -376,6 +377,17 @@ typedef struct VarCtx
 	int			ninner;
 	cbgpu_rel  *scanrel;		/* for scan-level Vars                                               */
 	int			scanrelid;
+	Owned	   *own;			/* where the code sets of string predicates are kept (scans only)    */
+	/* LIKE matches to launch once the whole scan has translated, so that a refusal never follows a launch */
+	struct
+	{
+		const cbgpu_dict *dict;
+		const char *pattern;
+		int32_t		len;
+		int32_t		bpchar_len;
+		uint32_t   *bits;
+	}			like[CBP_MAX_SETS];
+	int			nlike;
 } VarCtx;
 
 static int	translate(VarCtx *vc, const CbExpr *e, int *out);
@@ -446,6 +458,163 @@ translate_op(VarCtx *vc, const CbExpr *e, int *out)
 	return CBGPU_OK;
 }
 
+/* the dictionary behind `var`, a Var of this scan's relation whose column has one (`what` names the predicate in refusals) */
+static int
+scan_dict_column(VarCtx *vc, const CbExpr *var, const char *what, const cbgpu_dict **dict, int32_t *bpchar_len, int *pe)
+{
+	if (var->tag != T_CbVar || !vc->scanrel || !vc->own || var->varno == CB_OUTER_VAR || var->varno == CB_INNER_VAR)
+		return es_fail(vc->es, CBGPU_ERR_UNSUPPORTED, "%s is only taken over a column of the scan that evaluates it", what);
+	TRY(translate(vc, var, pe));
+	*dict = cbgpu_rel_dict(vc->scanrel, var->varattno - 1, bpchar_len);
+	if (!*dict)
+		return es_fail(vc->es, CBGPU_ERR_UNSUPPORTED, "%s over a column without a dictionary is not supported on the GPU path", what);
+	return CBGPU_OK;
+}
+
+/* a zero-filled device bitmap over the `n` codes of a dictionary, kept by the scan node, as code set *set of the stream */
+static int
+stream_add_set(VarCtx *vc, int32_t n, uint32_t **bits, int *set)
+{
+	CbPipeline *pl = &vc->s->pipe;
+	void	   *dev = NULL;
+
+	if (pl->nsets >= CBP_MAX_SETS || vc->own->ndevs >= MAX_OWNED)
+		return es_fail(vc->es, CBGPU_ERR_UNSUPPORTED, "more than %d string predicates in one pipeline", CBP_MAX_SETS);
+	GPU(vc->es, cbgpu_dev_alloc(vc->es->es_ctx, sizeof(uint32_t) * (size_t) ((n + 31) / 32 + 1), &dev));
+	vc->own->devs[vc->own->ndevs++] = dev;
+	*bits = dev;
+	*set = pl->nsets++;
+	pl->sets[*set].bits = dev;
+	pl->sets[*set].nbits = n;
+	return CBGPU_OK;
+}
+
+/* col LIKE / NOT LIKE 'pattern' over a dictionary column: the pattern is matched once per distinct string on the device
+ * (k_dict_like), each row then tests its code's bit (INSET) */
+static int
+translate_like(VarCtx *vc, const CbExpr *e, int *out)
+{
+	const CbExpr *pat = e->nargs == 2 ? e->args[1] : NULL;
+	const cbgpu_dict *dict;
+	int32_t		bpchar_len;
+	uint32_t   *bits;
+	int			col,
+				set;
+
+	if (!pat)
+		return es_fail(vc->es, CBGPU_ERR_INVALID, "LIKE with %d arguments", e->nargs);
+	if (pat->tag != T_CbConst || pat->restype != CB_TEXT)
+		return es_fail(vc->es, CBGPU_ERR_UNSUPPORTED, "LIKE with a pattern other than a string constant is not supported on the GPU path");
+	if (pat->constisnull)
+		return es_fail(vc->es, CBGPU_ERR_UNSUPPORTED, "NULL constants are not supported on the GPU path");
+	if (pat->constlen < 0 || (pat->constlen > 0 && !pat->conststr))
+		return es_fail(vc->es, CBGPU_ERR_INVALID, "malformed string constant");
+	if (like_pattern_check((const uint8_t *) pat->conststr, pat->constlen))
+		return es_fail(vc->es, CBGPU_ERR_INVALID, "LIKE pattern must not end with escape character");
+	TRY(scan_dict_column(vc, e->args[0], "LIKE", &dict, &bpchar_len, &col));
+	if (bpchar_len < 0)
+		return es_fail(vc->es, CBGPU_ERR_UNSUPPORTED, "LIKE over a character(n) column whose n was not declared (cbgpu_rel_set_dict) "
+					   "is not supported on the GPU path");
+	TRY(stream_add_set(vc, cbgpu_dict_nentries(dict), &bits, &set));
+	vc->like[vc->nlike].dict = dict;
+	vc->like[vc->nlike].pattern = pat->conststr;
+	vc->like[vc->nlike].len = pat->constlen;
+	vc->like[vc->nlike].bpchar_len = bpchar_len;
+	vc->like[vc->nlike].bits = bits;
+	vc->nlike++;
+	*out = pe_op(vc->s, CBP_INSET, col, -1, CB_BOOL, 0, set);
+	if (*out >= 0 && e->op == CB_OP_NOTLIKE)
+		*out = pe_op(vc->s, CBP_NOT, *out, -1, CB_BOOL, 0, 0);
+	return *out < 0 ? es_fail(vc->es, CBGPU_ERR_UNSUPPORTED, "expression too large for the GPU path") : CBGPU_OK;
+}
+
+/* x IN (c1, c2, ...) (`=`, useOr) and x NOT IN (...) (`<>`, !useOr).  Over a dictionary column with string elements: the
+ * codes of the strings the column holds form a code set (INSET).  Otherwise the compares and OR / AND of the expansion
+ * ExecEvalScalarArrayOp evaluates (execExprInterp.c), through the ordinary operator translation. */
+static int
+translate_in_list(VarCtx *vc, const CbExpr *e, int *out)
+{
+	const int	in = e->op == CB_OP_EQ && e->useOr;
+	int			strings = 0;
+
+	if (e->nargs < 2)
+		return es_fail(vc->es, CBGPU_ERR_INVALID, "IN list without elements");
+	if (!in && !(e->op == CB_OP_NE && !e->useOr))
+		return es_fail(vc->es, CBGPU_ERR_UNSUPPORTED, "array comparison with operator %d and useOr %d is not supported on the GPU path",
+					   e->op, (int) e->useOr);
+	for (int i = 1; i < e->nargs; i++)
+	{
+		const CbExpr *c = e->args[i];
+
+		if (c->tag != T_CbConst)
+			return es_fail(vc->es, CBGPU_ERR_UNSUPPORTED, "IN list elements other than constants are not supported on the GPU path");
+		if (c->constisnull)
+			return es_fail(vc->es, CBGPU_ERR_UNSUPPORTED, "NULL constants are not supported on the GPU path");
+		if (c->restype == CB_TEXT && (c->constlen < 0 || (c->constlen > 0 && !c->conststr)))
+			return es_fail(vc->es, CBGPU_ERR_INVALID, "malformed string constant");
+		strings += c->restype == CB_TEXT;
+	}
+	if (strings)
+	{
+		const cbgpu_dict *dict;
+		int32_t		bpchar_len,
+					n;
+		uint32_t   *bits,
+				   *host;
+		int			col,
+					set,
+					rc;
+
+		if (strings != e->nargs - 1)
+			return es_fail(vc->es, CBGPU_ERR_UNSUPPORTED, "IN list mixing string and other constants");
+		TRY(scan_dict_column(vc, e->args[0], "an IN list of strings", &dict, &bpchar_len, &col));
+		n = cbgpu_dict_nentries(dict);
+		TRY(stream_add_set(vc, n, &bits, &set));
+		host = calloc((size_t) (n + 31) / 32 + 1, sizeof(uint32_t));
+		if (!host)
+			return es_fail(vc->es, CBGPU_ERR_NOMEM, "out of host memory");
+		/* bpchareq / texteq: cbgpu_dict_lookup compares as the column's type does; a string the column never holds adds no code */
+		for (int i = 1; i < e->nargs; i++)
+		{
+			const int32_t code = cbgpu_dict_lookup(dict, e->args[i]->conststr, e->args[i]->constlen);
+
+			if (code >= 0)
+				host[code >> 5] |= 1u << (code & 31);
+		}
+		rc = cbgpu_dev_write(vc->es->es_ctx, bits, sizeof(uint32_t) * (size_t) ((n + 31) / 32 + 1), host);
+		free(host);
+		if (rc != CBGPU_OK)
+			return es_fail(vc->es, rc, "%s", cbgpu_last_error(vc->es->es_ctx));
+		*out = pe_op(vc->s, CBP_INSET, col, -1, CB_BOOL, 0, set);
+		if (*out >= 0 && !in)
+			*out = pe_op(vc->s, CBP_NOT, *out, -1, CB_BOOL, 0, 0);
+		return *out < 0 ? es_fail(vc->es, CBGPU_ERR_UNSUPPORTED, "expression too large for the GPU path") : CBGPU_OK;
+	}
+	{
+		int			acc = -1;
+
+		for (int i = 1; i < e->nargs; i++)
+		{
+			CbExpr	   *args[2] = {e->args[0], e->args[i]};
+			CbExpr		cmp;
+			int			r;
+
+			memset(&cmp, 0, sizeof(cmp));
+			cmp.tag = T_CbOpExpr;
+			cmp.restype = CB_BOOL;
+			cmp.op = e->op;
+			cmp.nargs = 2;
+			cmp.args = args;
+			TRY(translate_op(vc, &cmp, &r));
+			acc = acc < 0 ? r : pe_op(vc->s, in ? CBP_OR : CBP_AND, acc, r, CB_BOOL, 0, 0);
+			if (acc < 0)
+				return es_fail(vc->es, CBGPU_ERR_UNSUPPORTED, "expression too large for the GPU path");
+		}
+		*out = acc;
+		return CBGPU_OK;
+	}
+}
+
 static int
 translate(VarCtx *vc, const CbExpr *e, int *out)
 {
@@ -481,10 +650,16 @@ translate(VarCtx *vc, const CbExpr *e, int *out)
 		case T_CbConst:
 			if (e->constisnull)
 				return es_fail(vc->es, CBGPU_ERR_UNSUPPORTED, "NULL constants are not supported on the GPU path");
+			if (e->restype == CB_TEXT)
+				return es_fail(vc->es, CBGPU_ERR_UNSUPPORTED, "a string constant is only taken as a LIKE pattern or an IN list element");
 			*out = pe_const(s, e->restype, e->dscale, e->constval);
 			return CBGPU_OK;
 		case T_CbOpExpr:
+			if (e->op == CB_OP_LIKE || e->op == CB_OP_NOTLIKE)
+				return translate_like(vc, e, out);
 			return translate_op(vc, e, out);
+		case T_CbScalarArrayOpExpr:
+			return translate_in_list(vc, e, out);
 		case T_CbBoolExpr:
 			{
 				int			acc = -1;
@@ -540,7 +715,7 @@ emit_expr(CbEState *es, CbStream *s, int e)
 			TRY(emit_expr(es, s, x->l));
 			if (x->r >= 0)
 				TRY(emit_expr(es, s, x->r));
-			return emit_op(es, s, x->op, x->op == CBP_I2F ? (int) x->imm : 0, 0);
+			return emit_op(es, s, x->op, x->op == CBP_I2F || x->op == CBP_INSET ? (int) x->imm : 0, 0);
 		default:
 			return es_fail(es, CBGPU_ERR_INVALID, "cannot emit a transition state as a scalar");
 	}
@@ -968,6 +1143,7 @@ open_seqscan(CbPlanState *ps, CbStream **out)
 	vc.s = s;
 	vc.scanrel = rel;
 	vc.scanrelid = scan->scanrelid;
+	vc.own = &np(ps)->owned;
 	/* quals first (the AM evaluates pushed-down quals before fetching the remaining columns,
 	 * aocs_getnext_withqual, aocsam.c:1269): late materialisation falls out of program order */
 	for (int i = 0; i < ps->plan->nquals; i++)
@@ -977,6 +1153,9 @@ open_seqscan(CbPlanState *ps, CbStream **out)
 	s->nout = ps->plan->ntargets;
 	for (int i = 0; i < ps->plan->ntargets; i++)
 		TRY(translate(&vc, ps->plan->targetlist[i].expr, &s->out[i]));
+	for (int i = 0; i < vc.nlike; i++)
+		GPU(es, cbgpu_dict_match_like(es->es_ctx, vc.like[i].dict, vc.like[i].pattern, vc.like[i].len, vc.like[i].bpchar_len,
+									  vc.like[i].bits));
 	*out = s;
 	return CBGPU_OK;
 }
@@ -3262,6 +3441,56 @@ cb_ExecProcNodeBatch(CbPlanState *ps, cbgpu_rel **out)
 	return CBGPU_OK;
 }
 
+/* a LIKE or a string constant (a pattern, an IN list element) anywhere in the expression */
+static int
+expr_has_string_predicate(const CbExpr *e)
+{
+	if (!e)
+		return 0;
+	if ((e->tag == T_CbOpExpr && (e->op == CB_OP_LIKE || e->op == CB_OP_NOTLIKE)) || (e->tag == T_CbConst && e->restype == CB_TEXT))
+		return 1;
+	if (e->tag == T_CbOpExpr || e->tag == T_CbBoolExpr || e->tag == T_CbAggref || e->tag == T_CbScalarArrayOpExpr)
+		for (int i = 0; i < e->nargs; i++)
+			if (expr_has_string_predicate(e->args[i]))
+				return 1;
+	return 0;
+}
+
+static int
+exprs_have_string_predicate(CbExpr *const *es, int n)
+{
+	for (int i = 0; i < n; i++)
+		if (expr_has_string_predicate(es[i]))
+			return 1;
+	return 0;
+}
+
+/* whether one node's own expressions (not its children's) hold a string predicate */
+static int
+node_has_string_predicate(const CbPlan *node)
+{
+	for (int i = 0; i < node->ntargets; i++)
+		if (expr_has_string_predicate(node->targetlist[i].expr))
+			return 1;
+	if (exprs_have_string_predicate(node->qual, node->nquals))
+		return 1;
+	switch (node->type)
+	{
+		case T_CbHash:
+			return exprs_have_string_predicate(((const CbHash *) node)->hashkeys, ((const CbHash *) node)->nhashkeys);
+		case T_CbHashJoin:
+			{
+				const CbHashJoin *hj = (const CbHashJoin *) node;
+
+				return exprs_have_string_predicate(hj->hashkeys, hj->nhashkeys) || exprs_have_string_predicate(hj->joinqual, hj->njoinquals);
+			}
+		case T_CbMotion:
+			return exprs_have_string_predicate(((const CbMotion *) node)->hashExprs, ((const CbMotion *) node)->nhashExprs);
+		default:
+			return 0;
+	}
+}
+
 CbPlanState *
 cb_ExecInitNode(CbPlan *node, CbEState *estate, int eflags)
 {
@@ -3277,6 +3506,12 @@ cb_ExecInitNode(CbPlan *node, CbEState *estate, int eflags)
 		default:
 			es_fail(estate, CBGPU_ERR_UNSUPPORTED, "unrecognized / unsupported node type: %d", (int) node->type);	/* execProcnode.c:525 */
 			return NULL;
+	}
+	if (node->type != T_CbSeqScan && node_has_string_predicate(node))
+	{
+		/* refused here, before any child runs: a scan's stream translates its own quals, a join's come after its build side */
+		es_fail(estate, CBGPU_ERR_UNSUPPORTED, "LIKE and IN lists of strings are only taken in the quals of a scan on the GPU path");
+		return NULL;
 	}
 	ps = calloc(1, sizeof(CbPlanState));
 	ps->type = node->type;

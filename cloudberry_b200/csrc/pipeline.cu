@@ -46,8 +46,16 @@ cb_pipeline_to_dev(cbgpu_ctx *ctx, const CbPipeline *p, PipeDev *d, XProg *xp)
 	}
 	d->nops = p->nops;
 	memcpy(d->ops, p->ops, sizeof(CbpOp) * (size_t) p->nops);
+	if (p->nsets < 0 || p->nsets > CBP_MAX_SETS)
+		return cb_fail(ctx, CBGPU_ERR_INVALID, "pipeline declares %s%lld code sets", "", p->nsets);
+	for (int i = 0; i < p->nsets; i++)
 	{
-		const XAllow allow = {"pipeline", XM_PIPELINE_OPS, p->probes, p->nprobes, CBGPU_ERR_UNSUPPORTED};
+		if (p->sets[i].nbits < 0 || (p->sets[i].nbits > 0 && !p->sets[i].bits))
+			return cb_fail(ctx, CBGPU_ERR_INVALID, "pipeline code set %s%lld malformed", "", i);
+		d->sets[i] = p->sets[i];
+	}
+	{
+		const XAllow allow = {"pipeline", XM_PIPELINE_OPS, p->probes, p->nprobes, CBGPU_ERR_UNSUPPORTED, p->nsets};
 		const int	rc = xm_walk(ctx, allow, p->ncols, p->ops, p->nops, xp);
 
 		if (rc != CBGPU_OK)
@@ -600,6 +608,15 @@ k_pipeline_generic(const __grid_constant__ PipeDev P)
 						alive = false;
 					snull &= ~(1ull << sp);
 					break;
+				case CBP_INSET:
+					{
+						/* a NULL code stays NULL (its bit keeps the stack slot's NULL flag) */
+						const CbpSet &set = P.sets[a];
+						const int64_t v = st[sp - 1];
+
+						st[sp - 1] = alive && v >= 0 && v < set.nbits && ((set.bits[v >> 5] >> (v & 31)) & 1);
+						break;
+					}
 				default:
 					cbp_scalar_op(P.ops[pc], st, snull, sp, alive, P.status);
 					break;

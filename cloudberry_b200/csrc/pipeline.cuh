@@ -72,6 +72,7 @@ struct PipeDev
 	DProbe		probes[CBP_MAX_SRC - 1];
 	DSink		sink;
 	int		   *status;
+	CbpSet		sets[CBP_MAX_SETS];	/* code sets of INSET                                             */
 };
 
 /* one accumulator update of advance_aggregates (backend/executor/nodeAgg.c:856).  `args` are the

@@ -1396,7 +1396,7 @@ cb_try_probe_chain(cbgpu_ctx *ctx, const CbPipeline *p, const PipeDev *d, const 
 		PC_REJECT(2);
 	if (s->kind == CBP_SINK_PARTITION && s->nsegs > 64)
 		PC_REJECT(2);
-	if (x.f8ord)
+	if (x.f8ord || x.inset)
 		PC_REJECT(3);
 	memset(&P, 0, sizeof(P));
 	/* sections: quals (before the first probe only), then the probes in program order */

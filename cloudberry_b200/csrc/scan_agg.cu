@@ -518,7 +518,7 @@ try_small_agg(cbgpu_ctx *ctx, const CbPipeline *p, const PipeDev *d, const XProg
 	*handled = false;
 	if (s->kind != CBP_SINK_AGG || p->nprobes != 0 || p->drv_nsrc != 0 || s->nkeys > 2)
 		return CBGPU_OK;
-	if (x.f8ord || x.depth < s->nkeys)
+	if (x.f8ord || x.inset || x.depth < s->nkeys)
 		return CBGPU_OK;
 	memset(&P, 0, sizeof(P));
 	P.fspan = 0xFFFFFFFFu;		/* no qual: every value is inside the range */

@@ -32,6 +32,7 @@ struct XProg
 	int			stack[CBP_STACK];	/* node ids left on the stack at END: keys then args / outputs    */
 	int			depth;
 	bool		f8ord;			/* the program holds an F8ORD: float arithmetic stays with the generic kernel */
+	bool		inset;			/* the program holds an INSET: only the generic kernel reads code sets */
 };
 
 /* the values an op pops and pushes, internal fused ops (pipeline.cuh) included; PROBE pops its probe's keys */
@@ -48,7 +49,7 @@ xm_effect(const CbpOp &op, const CbpProbe *probes)
 	{
 		case CBP_LOAD: case CBP_CONST: case CBP_DUP: case XOP_MULCSUB:
 			return {0, 1};
-		case CBP_NOT: case CBP_I2F: case CBP_F8ORD:
+		case CBP_NOT: case CBP_I2F: case CBP_F8ORD: case CBP_INSET:
 			return {1, 1};
 		case CBP_FILTER: case CBP_POP:
 			return {1, 0};
@@ -63,8 +64,9 @@ xm_effect(const CbpOp &op, const CbpProbe *probes)
 
 /* opcodes as bits of XAllow.ops */
 #define XM_OP(c) (1u << (c))
-#define XM_PIPELINE_OPS (XM_OP(CBP_F8ORD + 1) - 1)	/* every CbpOpCode (F8ORD is the last) */
-#define XM_SCALAR_OPS (XM_PIPELINE_OPS & ~(XM_OP(CBP_FILTER) | XM_OP(CBP_PROBE) | XM_OP(CBP_END)))
+#define XM_PIPELINE_OPS (XM_OP(CBP_INSET + 1) - 1)	/* every CbpOpCode (INSET is the last) */
+/* join filters: no FILTER / PROBE / END, and no INSET (they take no code sets) */
+#define XM_SCALAR_OPS (XM_PIPELINE_OPS & ~(XM_OP(CBP_FILTER) | XM_OP(CBP_PROBE) | XM_OP(CBP_END) | XM_OP(CBP_INSET)))
 
 /* what a caller lets a program hold, and how it reports a refusal */
 struct XAllow
@@ -74,6 +76,7 @@ struct XAllow
 	const CbpProbe *probes;		/* PROBE a takes probes[a], a < nprobes                               */
 	int			nprobes;
 	int			too_deep;		/* the code of a stack deeper than CBP_STACK                          */
+	int			nsets;			/* INSET a takes code set a, a < nsets                                */
 };
 
 /* Checks a program of 1 .. CBP_MAX_OPS ops over `ncols` columns op by op and builds its expression trees in *x: FILTER and
@@ -87,6 +90,7 @@ xm_walk(cbgpu_ctx *ctx, const XAllow &allow, int ncols, const CbpOp *ops, int no
 	x->nsections = 0;
 	x->depth = 0;
 	x->f8ord = false;
+	x->inset = false;
 	for (int i = 0; i < nops; i++)
 	{
 		const CbpOp *op = &ops[i];
@@ -100,6 +104,8 @@ xm_walk(cbgpu_ctx *ctx, const XAllow &allow, int ncols, const CbpOp *ops, int no
 		if (op->code == CBP_PROBE && (op->a < 0 || op->a >= allow.nprobes || allow.probes[op->a].nkeys < 0 ||
 									  allow.probes[op->a].nkeys > CBP_MAX_KEYS))
 			return cb_fail(ctx, CBGPU_ERR_INVALID, "%s op %lld: bad PROBE", allow.what, i);
+		if (op->code == CBP_INSET && (op->a < 0 || op->a >= allow.nsets))
+			return cb_fail(ctx, CBGPU_ERR_INVALID, "%s op %lld: INSET of a code set the descriptor does not declare", allow.what, i);
 		if (op->code == CBP_END && i != nops - 1)
 			return cb_fail(ctx, CBGPU_ERR_INVALID, "%s op %lld: END before the last op", allow.what, i);
 		const XEffect e = xm_effect(*op, allow.probes);
@@ -133,6 +139,7 @@ xm_walk(cbgpu_ctx *ctx, const XAllow &allow, int ncols, const CbpOp *ops, int no
 				x->nodes[x->n] = {op->code, op->a, op->imm, e.pops > 0 ? x->stack[base] : -1, e.pops > 1 ? x->stack[base + 1] : -1};
 				x->stack[base] = x->n++;
 				x->f8ord |= op->code == CBP_F8ORD;
+				x->inset |= op->code == CBP_INSET;
 				break;
 		}
 		x->depth = base + e.pushes;

@@ -11,19 +11,20 @@ Host-side glue only: no compute happens here.
 import ctypes as C
 
 # ---- CbTypeId ----
-INT4, INT8, DATE, NUMERIC, BPCHAR1, DICT8, DICT32, FLOAT8, BOOL, NUMERIC128 = range(1, 11)
+INT4, INT8, DATE, NUMERIC, BPCHAR1, DICT8, DICT32, FLOAT8, BOOL, NUMERIC128, TEXT = range(1, 12)
 TYPE_WIDTH = {INT4: 4, INT8: 8, DATE: 4, NUMERIC: 8, BPCHAR1: 1, DICT8: 1, DICT32: 4, FLOAT8: 8, BOOL: 1, NUMERIC128: 16}
 TYPE_NAME = {INT4: "int4", INT8: "int8", DATE: "date", NUMERIC: "numeric", BPCHAR1: "bpchar1", DICT8: "dict8",
              DICT32: "dict32", FLOAT8: "float8", BOOL: "bool", NUMERIC128: "numeric128"}
 
 # ---- CbNodeTag ----
 T_SeqScan, T_Hash, T_HashJoin, T_Agg, T_Motion, T_LimitSort = range(100, 106)
-T_Var, T_Const, T_OpExpr, T_BoolExpr, T_Aggref = range(200, 205)
+T_Var, T_Const, T_OpExpr, T_BoolExpr, T_Aggref, T_ScalarArrayOpExpr = range(200, 206)
 
 INNER_VAR, OUTER_VAR = 65000, 65001
 
 OP_ADD, OP_SUB, OP_MUL = 1, 2, 3
 OP_EQ, OP_NE, OP_LT, OP_LE, OP_GT, OP_GE = 10, 11, 12, 13, 14, 15
+OP_LIKE, OP_NOTLIKE = 20, 21
 AND_EXPR, OR_EXPR, NOT_EXPR = 0, 1, 2
 AGG_COUNT_STAR, AGG_COUNT, AGG_SUM, AGG_AVG, AGG_MIN, AGG_MAX = 1, 2, 3, 4, 5, 6
 JOIN_INNER, JOIN_LEFT, JOIN_FULL, JOIN_RIGHT, JOIN_SEMI, JOIN_ANTI, JOIN_LASJ_NOTIN = range(7)
@@ -41,6 +42,7 @@ CbExpr._fields_ = [
     ("varno", C.c_int32), ("varattno", C.c_int32),
     ("constval", C.c_int64), ("constisnull", C.c_bool),
     ("op", C.c_int32), ("nargs", C.c_int32), ("args", C.POINTER(C.POINTER(CbExpr))),
+    ("conststr", C.c_char_p), ("constlen", C.c_int32), ("useOr", C.c_bool),
 ]
 
 
@@ -161,6 +163,34 @@ def OpExpr(op, a, b):
     e = CbExpr(tag=T_OpExpr, restype=typ, dscale=ds, op=op, nargs=2)
     e._keep = [a, b, _expr_array([a, b])]
     e.args = e._keep[2]
+    return e
+
+
+def TextConst(text):
+    """a string literal (CB_TEXT): a LIKE pattern or an IN list element"""
+    b = text if isinstance(text, bytes) else text.encode()
+    e = CbExpr(tag=T_Const, restype=TEXT, conststr=b, constlen=len(b))
+    e._keep = [b]
+    return e
+
+
+def Like(var, pattern, negate=False):
+    """var LIKE 'pattern' (~~), or NOT LIKE (!~~) with negate"""
+    p = pattern if isinstance(pattern, CbExpr) else TextConst(pattern)
+    e = CbExpr(tag=T_OpExpr, restype=BOOL, op=OP_NOTLIKE if negate else OP_LIKE, nargs=2)
+    e._keep = [var, p, _expr_array([var, p])]
+    e.args = e._keep[2]
+    return e
+
+
+def InList(var, elems, negate=False):
+    """var IN (e1, ...) = ScalarArrayOpExpr(=, useOr); NOT IN = (<>, not useOr).  Elements: CbExprs, or str (TextConst) /
+    int (a Const of var's type)"""
+    cs = [x if isinstance(x, CbExpr) else TextConst(x) if isinstance(x, (str, bytes)) else Const(var.restype, x, var.dscale)
+          for x in elems]
+    e = CbExpr(tag=T_ScalarArrayOpExpr, restype=BOOL, op=OP_NE if negate else OP_EQ, nargs=1 + len(cs), useOr=not negate)
+    e._keep = [var] + cs + [_expr_array([var] + cs)]
+    e.args = e._keep[-1]
     return e
 
 

@@ -40,7 +40,8 @@ typedef enum CbTypeId
 	CB_DICT32 = 7,		/* same, int32 code                                                       */
 	CB_FLOAT8 = 8,		/* double precision                IEEE binary64                          */
 	CB_BOOL = 9,		/* expression results only                                                */
-	CB_NUMERIC128 = 10	/* aggregate outputs: int128 scaled by 10^dscale (little endian lo,hi)    */
+	CB_NUMERIC128 = 10,	/* aggregate outputs: int128 scaled by 10^dscale (little endian lo,hi)    */
+	CB_TEXT = 11		/* a string literal (CbExpr.conststr): LIKE patterns, IN list elements    */
 } CbTypeId;
 
 static inline int
@@ -52,6 +53,7 @@ cb_type_width(CbTypeId t)
 		case CB_INT8: case CB_NUMERIC: case CB_FLOAT8: return 8;
 		case CB_BPCHAR1: case CB_DICT8: case CB_BOOL: return 1;
 		case CB_NUMERIC128: return 16;
+		case CB_TEXT: return 0;		/* constants only, never a column */
 	}
 	return 0;
 }
@@ -63,7 +65,8 @@ typedef enum CbNodeTag
 	/* plan nodes */
 	T_CbSeqScan = 100, T_CbHash, T_CbHashJoin, T_CbAgg, T_CbMotion, T_CbLimitSort,
 	/* expression nodes */
-	T_CbVar = 200, T_CbConst, T_CbOpExpr, T_CbBoolExpr, T_CbAggref
+	T_CbVar = 200, T_CbConst, T_CbOpExpr, T_CbBoolExpr, T_CbAggref,
+	T_CbScalarArrayOpExpr		/* primnodes.h ScalarArrayOpExpr: args[0] op ANY (useOr) / ALL (!useOr) of args[1 ..] */
 } CbNodeTag;
 
 /* special varnos (primnodes.h: INNER_VAR 65000, OUTER_VAR 65001) */
@@ -73,7 +76,8 @@ typedef enum CbNodeTag
 typedef enum CbOp
 {
 	CB_OP_ADD = 1, CB_OP_SUB, CB_OP_MUL,				/* int4/int8/numeric/float8 arithmetic     */
-	CB_OP_EQ = 10, CB_OP_NE, CB_OP_LT, CB_OP_LE, CB_OP_GT, CB_OP_GE	/* comparisons -> bool            */
+	CB_OP_EQ = 10, CB_OP_NE, CB_OP_LT, CB_OP_LE, CB_OP_GT, CB_OP_GE,	/* comparisons -> bool            */
+	CB_OP_LIKE = 20, CB_OP_NOTLIKE		/* ~~ / !~~ (textlike, bpcharlike): args (Var, CB_TEXT Const) */
 } CbOp;
 
 typedef enum CbBoolOp { CB_AND_EXPR = 0, CB_OR_EXPR, CB_NOT_EXPR } CbBoolOp;	/* primnodes.h BoolExprType */
@@ -104,6 +108,11 @@ typedef struct CbExpr
 	int32_t		op;			/* CbOp | CbBoolOp | CbAggFn                                              */
 	int32_t		nargs;
 	struct CbExpr **args;
+	/* T_CbConst of type CB_TEXT: the string's bytes (no terminator needed) */
+	const char *conststr;
+	int32_t		constlen;
+	/* T_CbScalarArrayOpExpr: true = ANY (x IN (...) is `=` with useOr), false = ALL (x NOT IN (...) is `<>` without) */
+	bool		useOr;
 } CbExpr;
 
 typedef struct CbTargetEntry

@@ -170,10 +170,22 @@ typedef enum CbpOpCode
 	CBP_PROBE,			/* a = probe index; pops that probe's key values (pushed in key order)        */
 	CBP_DUP,			/* push a copy of stack[a] (common sub-expressions)                           */
 	CBP_POP,
-	CBP_F8ORD			/* float8 bits -> an int64 whose integer order is float8's (float8_cmp_internal, utils/adt/float.c: every
+	CBP_F8ORD,			/* float8 bits -> an int64 whose integer order is float8's (float8_cmp_internal, utils/adt/float.c: every
 						 * NaN equal and above everything); its own inverse on non-NaN values.  Lets min / max(float8) use
 						 * the integer min / max accumulators */
+	CBP_INSET			/* a = code set (CbPipeline.sets); pop a dictionary code, push whether its bit is set: false for a code
+						 * outside [0, nbits), NULL for NULL.  LIKE / NOT LIKE / IN lists over dictionary columns.  Pipelines
+						 * only (not join filters); runs on the generic kernel */
 } CbpOpCode;
+
+#define CBP_MAX_SETS 4
+
+/* a set of dictionary codes: bit c of bits[c / 32] = code c is in the set */
+typedef struct CbpSet
+{
+	const uint32_t *bits;		/* device pointer, ceil(nbits / 32) words                             */
+	int32_t		nbits;
+} CbpSet;
 
 typedef struct CbpOp
 {
@@ -283,6 +295,8 @@ typedef struct CbPipeline
 	CbpProbe	probes[CBP_MAX_SRC - 1];
 	CbpSink		sink;
 	int32_t		force_generic;	/* tests: bypass the pattern-specialised kernels                      */
+	int32_t		nsets;			/* code sets INSET ops name                                           */
+	CbpSet		sets[CBP_MAX_SETS];
 } CbPipeline;
 
 int			cbgpu_pipeline_run(cbgpu_ctx *ctx, const CbPipeline *p);
@@ -553,11 +567,30 @@ int			cbgpu_aocs_dict_collect(cbgpu_ctx *ctx, const void *file_bytes, int64_t nb
 int			cbgpu_dict_finalize(cbgpu_dict *d, int32_t *nentries);
 /* entry `code` of a finalized dictionary: *text points at len bytes owned by the dictionary (no terminator) */
 int			cbgpu_dict_entry(const cbgpu_dict *d, int32_t code, const char **text, int32_t *len);
+/* entries of a finalized dictionary (0 before finalize); whether it has bpchar semantics */
+int32_t		cbgpu_dict_nentries(const cbgpu_dict *d);
+int32_t		cbgpu_dict_is_bpchar(const cbgpu_dict *d);
 /* code of a string (e.g. a Const of the plan), -1 when the column never holds it */
 int32_t		cbgpu_dict_lookup(const cbgpu_dict *d, const char *text, int32_t len);
 int			cbgpu_aocs_decode_dict_column(cbgpu_ctx *ctx, const void *file_bytes, int64_t nbytes, int32_t checksum,
 										  int32_t compresstype, int32_t typalign, const cbgpu_dict *dict, cbgpu_rel *rel,
 										  int32_t col, int64_t row_offset, int64_t *nrows);
+/* a finalized dictionary of n strings given on the host (texts[c], lens[c] bytes = code c): they must be distinct and in
+ * byte order, and for bpchar without trailing blanks; otherwise CBGPU_ERR_INVALID */
+int			cbgpu_dict_from_texts(cbgpu_ctx *ctx, int32_t n, const char *const *texts, const int32_t *lens, int32_t bpchar,
+								  cbgpu_dict **out);
+/* SQL LIKE (textlike / bpcharlike, utils/adt/like.c) of every entry against one pattern, on the device (k_dict_like): bit c of
+ * bits_dev[c / 32] = entry c matches; bits_dev has room for ceil(n / 32) words (nothing is written for an empty dictionary).
+ * bpchar_len = n >= 1 of a character(n) column, required for a bpchar dictionary (its entries are matched blank-padded to n
+ * characters), 0 for varchar / text; anything else, and a pattern that ends in a lone escape: CBGPU_ERR_INVALID, before any
+ * launch. */
+int			cbgpu_dict_match_like(cbgpu_ctx *ctx, const cbgpu_dict *dict, const char *pattern, int32_t len, int32_t bpchar_len,
+								  uint32_t *bits_dev);
+/* a relation column's dictionary (borrowed: the dictionary must outlive the relation) and the column's declared n for
+ * character(n), 0 for varchar / text.  cbgpu_aocs_decode_dict_column links the dictionary with n unknown (-1) for a bpchar
+ * dictionary, so a LIKE over the column is refused until this call gives n; cbgpu_rel_share_dict_hash passes the link on */
+int			cbgpu_rel_set_dict(cbgpu_rel *rel, int32_t col, const cbgpu_dict *dict, int32_t bpchar_len);
+const cbgpu_dict *cbgpu_rel_dict(const cbgpu_rel *rel, int32_t col, int32_t *bpchar_len);
 
 /* One row of the table's pg_aovisimap_<oid> for the segment file being loaded (access/appendonly/appendonly_visimap_entry.c:
  * AppendOnlyVisimapEntry_Copyout :196-262): first_row_no, and the detoasted `visimap` value after its varlena length
