@@ -1,6 +1,6 @@
 """Worker of tests/test_host_batched_pairs_fake_runtime.py: the host side of pair joins over a build side split into batches,
-driven over tests/native/fake_cudart.c (LD_PRELOADed by the test; kernels are no-ops, "device" memory is zeroed host memory).
-Prints one JSON object.  Not a test by itself."""
+driven over the no-op runtime of tests/fake_runtime.py (LD_PRELOADed by the test; kernels are no-ops, "device" memory is zeroed
+host memory).  Prints one JSON object.  Not a test by itself."""
 import ctypes as C
 import json
 import os
@@ -13,9 +13,6 @@ sys.path.insert(0, os.path.join(ROOT, "tests"))
 from cloudberry_b200 import capi  # noqa: E402
 from cloudberry_b200 import plan as P  # noqa: E402
 from cloudberry_b200.relation import HostRelation  # noqa: E402
-
-if os.environ.get("CB_TEST_LIBDIR"):
-    capi.HERE = os.environ["CB_TEST_LIBDIR"]        # libcbgpu.so (link) + a sanitizer build of libcbexec.so
 
 POLL = C.CFUNCTYPE(C.c_int, C.c_void_p)
 

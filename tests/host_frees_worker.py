@@ -1,6 +1,6 @@
-"""Worker of tests/test_host_frees_fake_runtime.py: makes every device allocation of a plan or of a library call fail in turn over
-tests/native/fake_cudart.c (LD_PRELOADed by the test; kernels are no-ops, "device" memory is zeroed host memory, and the runtime
-counts the device allocations still live).  Prints one JSON object.  Not a test by itself."""
+"""Worker of tests/test_host_frees_fake_runtime.py: makes every device allocation of a plan or of a library call fail in turn
+over the no-op runtime of tests/fake_runtime.py (LD_PRELOADed by the test; kernels are no-ops, "device" memory is zeroed host
+memory, and the runtime counts the device allocations still live).  Prints one JSON object.  Not a test by itself."""
 import ctypes as C
 import json
 import os
@@ -14,9 +14,6 @@ sys.path.insert(0, os.path.join(ROOT, "tests"))
 
 from cloudberry_b200 import capi, ssb, tpch  # noqa: E402
 from cloudberry_b200 import plan as P  # noqa: E402
-
-if os.environ.get("CB_TEST_LIBDIR"):
-    capi.HERE = os.environ["CB_TEST_LIBDIR"]        # sanitizer builds of libcbgpu.so and libcbexec.so
 
 fake = C.CDLL(None)
 fake.fake_cudart_fail_alloc_in.argtypes = [C.c_long]

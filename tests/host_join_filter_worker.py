@@ -1,6 +1,6 @@
 """Worker of tests/test_host_join_filter_fake_runtime.py: the host side of the pair probe (LEFT / SEMI / ANTI hash joins with a
-join filter, and INNER / FULL ones without) over tests/native/fake_cudart.c (LD_PRELOADed by the test; kernels are no-ops,
-"device" memory is zeroed host memory).  Prints one JSON object.  Not a test by itself."""
+join filter, and INNER / FULL ones without) over the no-op runtime of tests/fake_runtime.py (LD_PRELOADed by the test; kernels
+are no-ops, "device" memory is zeroed host memory).  Prints one JSON object.  Not a test by itself."""
 import ctypes as C
 import json
 import os
@@ -13,9 +13,6 @@ sys.path.insert(0, os.path.join(ROOT, "tests"))
 from cloudberry_b200 import capi  # noqa: E402
 from cloudberry_b200 import plan as P  # noqa: E402
 from host_batched_pairs_worker import dim, fact, scan  # noqa: E402
-
-if os.environ.get("CB_TEST_LIBDIR"):
-    capi.HERE = os.environ["CB_TEST_LIBDIR"]        # libcbgpu.so (link) + a sanitizer build of libcbexec.so
 
 POLL = C.CFUNCTYPE(C.c_int, C.c_void_p)
 JOINS = {"left": P.JOIN_LEFT, "semi": P.JOIN_SEMI, "anti": P.JOIN_ANTI, "right": P.JOIN_RIGHT, "full": P.JOIN_FULL,

@@ -1,5 +1,6 @@
-"""Worker of tests/test_host_logic_fake_runtime.py: drives the host executor over tests/native/fake_cudart.c (LD_PRELOADed by
-the test; kernels are no-ops, "device" memory is zeroed host memory).  Prints one JSON object.  Not a test by itself."""
+"""Worker of tests/test_host_logic_fake_runtime.py: drives the host executor over the no-op runtime of tests/fake_runtime.py
+(LD_PRELOADed by the test; kernels are no-ops, "device" memory is zeroed host memory).  Prints one JSON object.  Not a test by
+itself."""
 import json
 import os
 import sys
@@ -10,9 +11,6 @@ sys.path.insert(0, os.path.join(ROOT, "tests"))
 
 from cloudberry_b200 import capi, ssb, tpch  # noqa: E402
 from cloudberry_b200 import plan as P  # noqa: E402
-
-if os.environ.get("CB_TEST_LIBDIR"):
-    capi.HERE = os.environ["CB_TEST_LIBDIR"]        # libcbgpu.so (link) + a sanitizer build of libcbexec.so
 
 
 def main():

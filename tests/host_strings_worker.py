@@ -1,7 +1,7 @@
 """Worker of tests/test_host_string_predicates_fake_runtime.py: LIKE / NOT LIKE / IN lists through libcbexec.so and libcbgpu.so
-over tests/native/fake_cudart.c (LD_PRELOADed by the test; kernels are no-ops, "device" memory is zeroed host memory).  Records
-each refusal's code, message and kernel launches, which kernels each accepted plan launches, and what a failing device
-allocation leaves behind.  Prints one JSON object.  Not a test by itself."""
+over the no-op runtime of tests/fake_runtime.py (LD_PRELOADed by the test; kernels are no-ops, "device" memory is zeroed host
+memory).  Records each refusal's code, message and kernel launches, which kernels each accepted plan launches, and what a failing
+device allocation leaves behind.  Prints one JSON object.  Not a test by itself."""
 import ctypes as C
 import json
 import os

@@ -1,7 +1,7 @@
-"""Worker of tests/test_host_topn_fake_runtime.py: cbgpu_topn's host loop over tests/native/fake_cudart.c (LD_PRELOADed by the
-test; kernels are no-ops, "device" memory is zeroed host memory, so every key reads back as constant and each call goes to the
-tournament).  Prints one "TOPN {json}" line per call as soon as the call returns, so that a call that never returns is named by
-the lines before it.  Not a test by itself.
+"""Worker of tests/test_host_topn_fake_runtime.py: cbgpu_topn's host loop over the no-op runtime of tests/fake_runtime.py
+(LD_PRELOADed by the test; kernels are no-ops, "device" memory is zeroed host memory, so every key reads back as constant and
+each call goes to the tournament).  Prints one "TOPN {json}" line per call as soon as the call returns, so that a call that never
+returns is named by the lines before it.  Not a test by itself.
 
     host_topn_worker.py calls N      every LIMIT 1..64 over N rows, with 1 and with 4 keys
     host_topn_worker.py refusals     the calls cbgpu_topn must refuse before any launch"""

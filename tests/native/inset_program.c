@@ -1,9 +1,9 @@
 /*
- * inset_program.c - pipeline descriptors holding CBP_INSET, handed to cbgpu_pipeline_run over tests/native/fake_cudart.c, for
- * tests/test_host_string_predicates_fake_runtime.py.  Shapes the fused kernels take (TPC-H Q1 for the small scan-aggregate
- * kernel, Q3 for the probe chain) with an INSET computed and dropped on the way must run on the generic kernel, which is the
- * only one that reads code sets; an INSET naming a set the descriptor does not declare, and a malformed set, are refused
- * before any launch; a join filter takes no INSET.  Prints one line per case:
+ * inset_program.c - pipeline descriptors holding CBP_INSET, handed to cbgpu_pipeline_run over the no-op runtime of
+ * tests/fake_runtime.py, for tests/test_host_string_predicates_fake_runtime.py.  Shapes the fused kernels take (TPC-H Q1 for the
+ * small scan-aggregate kernel, Q3 for the probe chain) with an INSET computed and dropped on the way must run on the generic
+ * kernel, which is the only one that reads code sets; an INSET naming a set the descriptor does not declare, and a malformed
+ * set, are refused before any launch; a join filter takes no INSET.  Prints one line per case:
  *   <name> <return code> <kernels launched> <kernel name, or the error message>
  */
 #include <stdio.h>

@@ -1,8 +1,8 @@
 /*
  * pipeline_program.c - pipeline descriptors built in C and handed to cbgpu_pipeline_run, for
  * tests/test_host_pipeline_program_fake_runtime.py.  Each malformed postfix program must be refused with its code before any
- * launch; each valid one must reach the kernel its shape calls for.  Runs over tests/native/fake_cudart.c (LD_PRELOADed: no
- * kernel computes anything, only the host side is under test).  Prints one line per case:
+ * launch; each valid one must reach the kernel its shape calls for.  Runs over the no-op runtime of tests/fake_runtime.py
+ * (LD_PRELOADed: no kernel computes anything, only the host side is under test).  Prints one line per case:
  *   <name> <return code> <kernels launched> <kernel name, or the error message>
  */
 #include <stdio.h>

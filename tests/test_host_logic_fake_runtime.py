@@ -1,7 +1,7 @@
 """The host side of the product without a GPU (not gpu): libcbexec.so + the host code of libcbgpu.so run over a CUDA runtime
-that computes nothing (tests/native/fake_cudart.c, LD_PRELOADed into a subprocess: zeroed host memory as "device" memory,
-kernel launches are no-ops).  No result can come out of that - every query returns zero rows, which the test asserts - but
-everything the host does around the kernels is exercised: Plan -> stream translation, pipeline program emission, the
+that computes nothing (the no-op runtime of tests/fake_runtime.py, LD_PRELOADed into a subprocess: zeroed host memory as
+"device" memory, kernel launches are no-ops).  No result can come out of that - every query returns zero rows, which the test
+asserts - but everything the host does around the kernels is exercised: Plan -> stream translation, pipeline program emission, the
 specialised-kernel matcher, Motions inside a 3-segment cluster, launch bookkeeping, read-back, clean-up, the segment file loader's file handling (naming, EOFs, missing files), and the refusals
 (HAVING, sorted aggregation, Sort without LIMIT, RIGHT join, numeric join keys, a scanrelid outside the range table) with the
 error code and message a caller sees.  Run twice: as built, and with libcbexec.so rebuilt under AddressSanitizer + UBSan."""
@@ -10,30 +10,9 @@ import os
 import subprocess
 import sys
 
-import pytest
-
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-CUDA_INC = "/usr/local/cuda/include"
-pytestmark = pytest.mark.skipif(not os.path.exists(os.path.join(CUDA_INC, "cuda_runtime_api.h")), reason="needs the CUDA headers")
+from fake_runtime import ROOT, fake_cudart, run_worker
 
 UNSUPPORTED, INVALID, NOMEM = -3, -2, -5
-
-
-@pytest.fixture(scope="module")
-def fake(tmp_path_factory):
-    d = tmp_path_factory.mktemp("fakecuda")
-    so = str(d / "libfakecudart.so")
-    subprocess.check_call(["gcc", "-O1", "-g", "-shared", "-fPIC", "-Wall", "-Werror", "-I" + CUDA_INC, "-o", so,
-                           os.path.join(ROOT, "tests", "native", "fake_cudart.c")])
-    return d, so
-
-
-def _run(env):
-    p = subprocess.run([sys.executable, os.path.join(ROOT, "tests", "host_logic_worker.py")], capture_output=True, text=True,
-                       timeout=600, env=dict(os.environ, **env))
-    lines = [ln for ln in p.stdout.splitlines() if ln.startswith("HOSTLOGIC ")]
-    assert p.returncode == 0 and lines, (p.stdout[-2000:], p.stderr[-4000:])
-    return json.loads(lines[0][len("HOSTLOGIC "):])
 
 
 def _check(out):
@@ -84,64 +63,32 @@ def _check(out):
     assert de["raised"] >= 4 and {-4, -6, -5} <= set(de["codes"]) and all(-6 <= c < 0 for c in de["codes"])
 
 
-def test_host_executor_over_a_runtime_that_computes_nothing(fake):
-    _, so = fake
-    _check(_run({"LD_PRELOAD": so}))
+def test_host_executor_over_a_runtime_that_computes_nothing():
+    _check(run_worker("host_logic_worker", "HOSTLOGIC")[0])
 
 
-def test_the_same_under_address_and_ub_sanitizers(fake):
-    d, so = fake
-    asan = subprocess.check_output(["gcc", "-print-file-name=libasan.so"], text=True).strip()
-    if not os.path.exists(asan):
-        pytest.skip("no libasan")
-    libdir = str(d)
-    src = os.path.join(ROOT, "cloudberry_b200", "csrc", "exec")
-    os.symlink(os.path.join(ROOT, "cloudberry_b200", "libcbgpu.so"), os.path.join(libdir, "libcbgpu.so"))
-    subprocess.check_call(["gcc", "-O1", "-g", "-fPIC", "-shared", "-fsanitize=address,undefined", "-fno-sanitize-recover=undefined",
-                           "-o", os.path.join(libdir, "libcbexec.so")] +
-                          [os.path.join(src, f) for f in ("cb_exec.c", "cb_numeric.c", "cb_aocs_load.c", "cb_tupser.c")] +
-                          ["-L" + libdir, "-lcbgpu", "-Wl,-rpath," + libdir])
-    _check(_run({"LD_PRELOAD": asan + ":" + so, "ASAN_OPTIONS": "detect_leaks=0", "CB_TEST_LIBDIR": libdir}))
+def test_the_same_under_address_and_ub_sanitizers():
+    _check(run_worker("host_logic_worker", "HOSTLOGIC", sanitized="exec")[0])
 
 
-def test_storage_side_host_walk_under_sanitizers(fake, tmp_path):
+def test_storage_side_host_walk_under_sanitizers():
     """BOTH libraries rebuilt with AddressSanitizer + UBSan on their host code (the .cu files' host half through nvcc
     -Xcompiler): the plan shapes again, then cbgpu_aocs_decode_column's block header walk over every reference-written golden
     column file (plain, RLE / delta, zlib, zstd) and 40 damaged copies of each from exact-size buffers"""
-    import shutil
-    _, so = fake
-    nvcc = shutil.which("nvcc") or "/usr/local/cuda/bin/nvcc"
-    asan = subprocess.check_output(["gcc", "-print-file-name=libasan.so"], text=True).strip()
-    if not (os.path.exists(nvcc) and os.path.exists(asan)):
-        pytest.skip("needs nvcc and libasan")
-    tree = tmp_path / "tree"
-    shutil.copytree(os.path.join(ROOT, "cloudberry_b200", "csrc"), tree / "cloudberry_b200" / "csrc",
-                    ignore=shutil.ignore_patterns("*.o"))
-    shutil.copytree(os.path.join(ROOT, "include"), tree / "include")
-    san = "-Xcompiler -fsanitize=address -Xcompiler -fsanitize=undefined -Xcompiler -fno-omit-frame-pointer"
-    subprocess.check_call(["make", "-s", "-j8", "-C", str(tree / "cloudberry_b200" / "csrc"), "../libcbgpu.so",
-                           "ARCH=-gencode arch=compute_90a,code=sm_90a " + san])
-    libdir = str(tree / "cloudberry_b200")
-    src = os.path.join(ROOT, "cloudberry_b200", "csrc", "exec")
-    subprocess.check_call(["gcc", "-O1", "-g", "-fPIC", "-shared", "-fsanitize=address,undefined", "-fno-sanitize-recover=undefined",
-                           "-o", os.path.join(libdir, "libcbexec.so")] +
-                          [os.path.join(src, f) for f in ("cb_exec.c", "cb_numeric.c", "cb_aocs_load.c", "cb_tupser.c")] +
-                          ["-L" + libdir, "-lcbgpu", "-Wl,-rpath," + libdir])
-    out = _run({"LD_PRELOAD": asan + ":" + so, "ASAN_OPTIONS": "detect_leaks=0", "CB_TEST_LIBDIR": libdir, "CB_TEST_AOCS_FUZZ": "40"})
+    out = run_worker("host_logic_worker", "HOSTLOGIC", sanitized="both", env={"CB_TEST_AOCS_FUZZ": "40"})[0]
     _check(out)
     assert out["aocs_fuzz"]["calls"] > 1000 and out["aocs_fuzz"]["errors"] > 100
 
 
-def test_bench_main_arm_control_flow(fake, tmp_path):
+def test_bench_main_arm_control_flow(tmp_path):
     """bench.py's GPU arm from argument parsing to the JSON line, over the no-op runtime at a small scale factor: the numbers
     mean nothing (no kernel runs), the contract's keys and their bookkeeping do - steps, warm-up, launches counted, the e2e
     leg's byte counts, the q3 / q5 lines, one --dump-outputs file per timed query.  (The CPU legs have their own test,
     tests/test_bench_cpu.py.)"""
-    _, so = fake
     dump = tmp_path / "out"
     p = subprocess.run([sys.executable, os.path.join(ROOT, "bench.py"), "--sf", "0.05", "--steps", "2", "--warmup", "3", "--no-cpu",
                         "--dump-outputs", str(dump)],
-                       capture_output=True, text=True, timeout=600, env=dict(os.environ, LD_PRELOAD=so), cwd=ROOT)
+                       capture_output=True, text=True, timeout=600, env=dict(os.environ, LD_PRELOAD=fake_cudart()), cwd=ROOT)
     lines = [ln for ln in p.stdout.splitlines() if ln.startswith("{")]
     assert p.returncode == 0 and len(lines) == 1, (p.stdout[-2000:], p.stderr[-3000:])
     line = json.loads(lines[0])
@@ -165,19 +112,18 @@ def test_bench_main_arm_control_flow(fake, tmp_path):
     assert sorted(os.listdir(dump)) == ["q1.npy", "q3.npy", "q5.npy", "ssb_q4_1.npy", "ssb_q4_2.npy", "ssb_q4_3.npy"]
 
 
-def test_bench_result_check_bites(fake, tmp_path):
+def test_bench_result_check_bites(tmp_path):
     """with golden rows for the configuration at hand, a run whose kernels compute nothing must FAIL: bench.py prints its line with
     result_check = MISMATCH and exits 1"""
     import multiprocessing as mp
     sys.path.insert(0, os.path.join(ROOT, "tools"))
     import make_bench_golden as G
-    _, so = fake
     with mp.Pool(2) as pool:
         gold = {"q1_sf0.05": G.run_q1(pool, 0.05, 1), "q3_sf0.05": G.run_q3(pool, 0.05), "q5_sf0.05": G.run_q5(pool, 0.05)}
     path = tmp_path / "gold.json"
     path.write_text(json.dumps(gold))
     p = subprocess.run([sys.executable, os.path.join(ROOT, "bench.py"), "--sf", "0.05", "--steps", "2", "--warmup", "3", "--no-cpu", "--no-e2e", "--no-ssb"],
-                       capture_output=True, text=True, timeout=600, env=dict(os.environ, LD_PRELOAD=so, CBGPU_BENCH_GOLDEN=str(path)), cwd=ROOT)
+                       capture_output=True, text=True, timeout=600, env=dict(os.environ, LD_PRELOAD=fake_cudart(), CBGPU_BENCH_GOLDEN=str(path)), cwd=ROOT)
     lines = [ln for ln in p.stdout.splitlines() if ln.startswith("{")]
     assert p.returncode == 1 and len(lines) == 1, (p.returncode, p.stdout[-2000:], p.stderr[-2000:])
     line = json.loads(lines[0])
@@ -185,11 +131,10 @@ def test_bench_result_check_bites(fake, tmp_path):
     assert "result_check FAILED" in p.stderr
 
 
-def test_smoke_cannot_pass_without_real_kernels(fake):
+def test_smoke_cannot_pass_without_real_kernels():
     """__graft_entry__.smoke() compares the device's rows with the oracle's and the reference's expected rows: over a runtime
     whose kernels do nothing it must fail - it is a check of results, not of plumbing"""
-    _, so = fake
     p = subprocess.run([sys.executable, "-c", "import __graft_entry__ as g; g.smoke()"], capture_output=True, text=True, timeout=600,
-                       env=dict(os.environ, LD_PRELOAD=so), cwd=ROOT)
+                       env=dict(os.environ, LD_PRELOAD=fake_cudart()), cwd=ROOT)
     assert p.returncode != 0 and "AssertionError" in p.stderr, (p.stdout[-500:], p.stderr[-1500:])
     assert "smoke ok" not in p.stdout

@@ -1,19 +1,12 @@
 """The postfix program of a pipeline descriptor, checked on the host (not gpu): tests/native/pipeline_program.c builds CbPipeline
-descriptors in C and calls cbgpu_pipeline_run over tests/native/fake_cudart.c, a CUDA runtime that computes nothing
-(LD_PRELOADed, as test_host_frees_fake_runtime.py does).  Every malformed program is refused with its code before anything is
+descriptors in C and calls cbgpu_pipeline_run over the no-op runtime of tests/fake_runtime.py, a CUDA runtime that computes
+nothing (LD_PRELOADed).  Every malformed program is refused with its code before anything is
 launched; a program whose stack reaches exactly CBP_STACK values runs; each valid shape goes to the kernel that fuses it, or to
 the generic kernel when a matcher must decline it (float8 order keys, a qual behind a probe, a NE qual, an empty qual range).
 Run twice: as built, and with libcbgpu.so and the driver rebuilt under AddressSanitizer + UBSan."""
-import os
 import re
-import shutil
-import subprocess
 
-import pytest
-
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-CUDA_INC = "/usr/local/cuda/include"
-pytestmark = pytest.mark.skipif(not os.path.exists(os.path.join(CUDA_INC, "cuda_runtime_api.h")), reason="needs the CUDA headers")
+from fake_runtime import run_driver
 
 INVALID, UNSUPPORTED = -2, -3
 SMALL_AGG, PROBE_CHAIN, GENERIC = "k_scan_agg_small<", "k_probe_chain", "k_pipeline_generic"
@@ -32,32 +25,6 @@ ROUTES = {"q1": SMALL_AGG, "q1_f8ord": GENERIC, "q1_ne": GENERIC, "q1_empty": GE
           "q3_byte_empty": GENERIC}
 
 
-@pytest.fixture(scope="module")
-def fake(tmp_path_factory):
-    d = tmp_path_factory.mktemp("fakecuda")
-    so = str(d / "libfakecudart.so")
-    subprocess.check_call(["gcc", "-O1", "-g", "-shared", "-fPIC", "-Wall", "-Werror", "-I" + CUDA_INC, "-o", so,
-                           os.path.join(ROOT, "tests", "native", "fake_cudart.c")])
-    return so
-
-
-def _driver(exe, libdir, flags=()):
-    subprocess.check_call(["gcc", "-O1", "-g", "-Wall", "-Werror", *flags, "-I" + os.path.join(ROOT, "include"), "-o", exe,
-                           os.path.join(ROOT, "tests", "native", "pipeline_program.c"), "-L" + libdir, "-lcbgpu",
-                           "-Wl,-rpath," + libdir])
-
-
-def _run(exe, env):
-    p = subprocess.run([exe], capture_output=True, text=True, timeout=600, env=dict(os.environ, **env))
-    assert p.returncode == 0, (p.stdout[-2000:], p.stderr[-4000:])
-    assert "runtime error" not in p.stderr and "AddressSanitizer" not in p.stderr, p.stderr[-4000:]
-    out = {}
-    for ln in p.stdout.splitlines():
-        name, code, launches, what = (ln.split(" ", 3) + [""])[:4]
-        out[name] = {"code": int(code), "launches": int(launches), "what": what}
-    return out
-
-
 def _check(out):
     assert set(out) == set(REFUSED) | set(ROUTES) | {"depth_48"}, sorted(out)
     for name, code in REFUSED.items():
@@ -71,24 +38,9 @@ def _check(out):
         assert r["code"] == 0 and r["launches"] > 0 and r["what"].startswith(kernel), (name, r)
 
 
-def test_pipeline_programs_over_a_runtime_that_computes_nothing(fake, tmp_path):
-    exe = str(tmp_path / "pipeline_program")
-    libdir = os.path.join(ROOT, "cloudberry_b200")
-    _driver(exe, libdir)
-    _check(_run(exe, {"LD_PRELOAD": fake}))
+def test_pipeline_programs_over_a_runtime_that_computes_nothing():
+    _check(run_driver("pipeline_program"))
 
 
-def test_the_same_under_address_and_ub_sanitizers(fake, tmp_path):
-    nvcc = shutil.which("nvcc") or "/usr/local/cuda/bin/nvcc"
-    asan = subprocess.check_output(["gcc", "-print-file-name=libasan.so"], text=True).strip()
-    if not (os.path.exists(nvcc) and os.path.exists(asan)):
-        pytest.skip("needs nvcc and libasan")
-    tree = tmp_path / "tree"
-    shutil.copytree(os.path.join(ROOT, "cloudberry_b200", "csrc"), tree / "cloudberry_b200" / "csrc", ignore=shutil.ignore_patterns("*.o"))
-    shutil.copytree(os.path.join(ROOT, "include"), tree / "include")
-    san = "-Xcompiler -fsanitize=address -Xcompiler -fsanitize=undefined -Xcompiler -fno-omit-frame-pointer"
-    subprocess.check_call(["make", "-s", "-j8", "-C", str(tree / "cloudberry_b200" / "csrc"), "../libcbgpu.so",
-                           "ARCH=-gencode arch=compute_90a,code=sm_90a " + san])
-    exe = str(tmp_path / "pipeline_program")
-    _driver(exe, str(tree / "cloudberry_b200"), ("-fsanitize=address,undefined", "-fno-sanitize-recover=undefined"))
-    _check(_run(exe, {"LD_PRELOAD": asan + ":" + fake, "ASAN_OPTIONS": "detect_leaks=0"}))
+def test_the_same_under_address_and_ub_sanitizers():
+    _check(run_driver("pipeline_program", sanitized=True))

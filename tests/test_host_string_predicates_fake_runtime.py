@@ -1,5 +1,5 @@
-"""String predicates on the host side (not gpu): libcbgpu.so and libcbexec.so over tests/native/fake_cudart.c, a CUDA runtime
-that computes nothing and counts the device allocations still live (LD_PRELOADed into subprocesses).
+"""String predicates on the host side (not gpu): libcbgpu.so and libcbexec.so over the no-op runtime of tests/fake_runtime.py, a
+CUDA runtime that computes nothing and counts the device allocations still live (LD_PRELOADed into subprocesses).
 
 - tests/host_strings_worker.py: every refusal of LIKE / NOT LIKE / IN lists comes with its code and message before any kernel
   launch, also when a later predicate of the same scan is the one refused and when the predicate sits above a join; a
@@ -8,16 +8,7 @@ that computes nothing and counts the device allocations still live (LD_PRELOADed
   every device allocation of the new library calls and plans failing in turn leaves nothing allocated.
 - tests/native/inset_program.c: shapes the fused kernels take go to the generic kernel once they hold an INSET; INSET
   descriptors with a missing or malformed set, and join filters with an INSET, are refused before any launch."""
-import json
-import os
-import subprocess
-import sys
-
-import pytest
-
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-CUDA_INC = "/usr/local/cuda/include"
-pytestmark = pytest.mark.skipif(not os.path.exists(os.path.join(CUDA_INC, "cuda_runtime_api.h")), reason="needs the CUDA headers")
+from fake_runtime import run_driver, run_worker
 
 INVALID, UNSUPPORTED, NOMEM = -2, -3, -5
 REFUSED = {"malformed_pattern": (INVALID, "must not end with escape character"),
@@ -52,21 +43,8 @@ PROGRAMS = {"q1": (0, "k_scan_agg_small<"), "q1_inset": (0, "k_pipeline_generic"
             "set_negative_size": (INVALID, "code set 0 malformed"), "join_filter_inset": (INVALID, "join filter op 1")}
 
 
-@pytest.fixture(scope="module")
-def fake(tmp_path_factory):
-    d = tmp_path_factory.mktemp("fakecuda")
-    so = str(d / "libfakecudart.so")
-    subprocess.check_call(["gcc", "-O1", "-g", "-shared", "-fPIC", "-Wall", "-Werror", "-I" + CUDA_INC, "-o", so,
-                           os.path.join(ROOT, "tests", "native", "fake_cudart.c")])
-    return so
-
-
-def test_executor_and_library_calls(fake):
-    p = subprocess.run([sys.executable, os.path.join(ROOT, "tests", "host_strings_worker.py")], capture_output=True, text=True,
-                       timeout=1200, env=dict(os.environ, LD_PRELOAD=fake))
-    lines = [ln for ln in p.stdout.splitlines() if ln.startswith("HOSTSTRINGS ")]
-    assert p.returncode == 0 and lines, (p.stdout[-2000:], p.stderr[-4000:])
-    out = json.loads(lines[0][len("HOSTSTRINGS "):])
+def test_executor_and_library_calls():
+    out = run_worker("host_strings_worker", "HOSTSTRINGS", timeout=1200)[0]
     for name, (code, msg) in REFUSED.items():
         r = out["refused"][name]
         assert r["code"] == code and msg in r["msg"] and r["launches"] == 0, (name, r)
@@ -81,17 +59,8 @@ def test_executor_and_library_calls(fake):
     assert out["calls"]["dict_from_texts"]["failed"] >= 4
 
 
-def test_inset_descriptors(fake, tmp_path):
-    exe = str(tmp_path / "inset_program")
-    libdir = os.path.join(ROOT, "cloudberry_b200")
-    subprocess.check_call(["gcc", "-O1", "-g", "-Wall", "-Werror", "-I" + os.path.join(ROOT, "include"), "-o", exe,
-                           os.path.join(ROOT, "tests", "native", "inset_program.c"), "-L" + libdir, "-lcbgpu", "-Wl,-rpath," + libdir])
-    p = subprocess.run([exe], capture_output=True, text=True, timeout=600, env=dict(os.environ, LD_PRELOAD=fake))
-    assert p.returncode == 0, (p.stdout[-2000:], p.stderr[-4000:])
-    got = {}
-    for ln in p.stdout.splitlines():
-        name, code, launches, what = (ln.split(" ", 3) + [""])[:4]
-        got[name] = (int(code), int(launches), what)
+def test_inset_descriptors():
+    got = {name: (r["code"], r["launches"], r["what"]) for name, r in run_driver("inset_program").items()}
     assert set(got) == set(PROGRAMS)
     for name, (code, what) in PROGRAMS.items():
         c, n, w = got[name]
