@@ -222,12 +222,10 @@ agg_snapshot_block(const AggDev &t, AggSnap *out)
 void		cb_agg_adopt_snapshot(cbgpu_aggtable *t, const AggSnap *snap);
 
 
-#ifdef __CUDACC__
-#define CB_HD_DECL __host__ __device__ __forceinline__
-#else
-#define CB_HD_DECL static inline
-#endif
-/* join hash table, device view: slot = hash32 << 32 | rowid32, EMPTY = ~0 */
+#define CB_HD __host__ __device__ __forceinline__
+
+/* join hash table, device view.  The slot format is owned by the ht_slot_* / ht_probe_tag / ht_tag_match helpers below and
+ * ht_slot_match / ht_find further down: every build and probe goes through them. */
 #define HT_EMPTY 0xFFFFFFFFFFFFFFFFull
 struct HtDev
 {
@@ -259,17 +257,50 @@ struct HtDev
 	int32_t		batch_id;
 };
 
-CB_HD_DECL bool
+CB_HD bool
 ht_in_batch(int32_t nbatch, int32_t batch_shift, int32_t batch_id, uint32_t hash)
 {
 	return nbatch <= 1 || (int32_t) (hash >> batch_shift) == batch_id;
 }
 
 /* is an outer key value inside a key-in-slot table's domain?  Outside it nothing can match. */
-CB_HD_DECL bool
+CB_HD bool
 ht_key_in_domain(int32_t keyslot, int64_t key)
 {
 	return keyslot == 1 ? key == (int64_t) (int32_t) key : (uint64_t) key <= 0xFFFFFFFFull;
+}
+
+/* A slot is tag32 << 32 | row32, HT_EMPTY = ~0, probed linearly from hash & mask.  The tag is the key itself in a key-in-slot
+ * table (keyslot 1 or 2: a tag match is a key match, given ht_key_in_domain), and the key hash otherwise (a tag match is
+ * confirmed by the build row's key columns).  The build side tags its rows with the same function a probe compares with. */
+CB_HD uint32_t
+ht_probe_tag(int32_t keyslot, uint32_t hash, int64_t key0)
+{
+	return keyslot ? (uint32_t) key0 : hash;
+}
+
+CB_HD unsigned long long
+ht_slot_entry(uint32_t tag, uint32_t row)
+{
+	return ((unsigned long long) tag << 32) | row;
+}
+
+CB_HD bool
+ht_slot_empty(unsigned long long e)
+{
+	return e == HT_EMPTY;
+}
+
+CB_HD uint32_t
+ht_slot_row(unsigned long long e)
+{
+	return (uint32_t) e;
+}
+
+CB_HD bool
+ht_tag_match(unsigned long long e, uint32_t tag)
+{
+	return (uint32_t) (e >> 32) == tag;
 }
 
 struct cbgpu_hashtable
@@ -431,7 +462,6 @@ cb_type_w(int t)
 /* ---------------------------------------------------------------------------------------------
  * the reference's hash functions, device + host
  * --------------------------------------------------------------------------------------------- */
-#define CB_HD __host__ __device__ __forceinline__
 
 CB_HD uint32_t
 pg_rot(uint32_t x, int k)
@@ -822,6 +852,63 @@ cb_load_widen(const void *data, int type, uint32_t row)
 			return (int64_t) __ldg((const uint8_t *) data + row);
 	}
 }
+
+#ifdef __CUDACC__
+/* the join-table hash of a row's keys is h = 0 folded with each key in turn: h = jh_key_fold(h, type, value, dict).  Build and
+ * probe sides must agree on it bit for bit (the int4 / int8 fast forms of probe_chain.cu are this fold over one key). */
+__device__ __forceinline__ uint32_t
+jh_key_fold(uint32_t h, int type, int64_t v, const uint32_t *dict)
+{
+	return pg_hash_combine(h, jh_hash_datum(type, v, dict), false);
+}
+
+/* does slot entry e hold a build row whose key equals the probe's?  Tag first, then (unless the table is key-in-slot) the
+ * build row's key columns by row id */
+__device__ __forceinline__ bool
+ht_slot_match(const HtDev &ht, unsigned long long e, uint32_t tag, const int64_t *key, int nkeys)
+{
+	if (!ht_tag_match(e, tag))
+		return false;
+	for (int k = 0; k < nkeys && !ht.keyslot; k++)
+		if (cb_load_widen(ht.keydata[k], ht.keytype[k], ht_slot_row(e)) != key[k])
+			return false;
+	return true;
+}
+
+/* slot `pos` of a table: LDG, through the read-only cache (the table in global memory); else a plain load through a generic
+ * pointer, global or shared memory (a CTA's copy of a small table) */
+template <bool LDG>
+__device__ __forceinline__ unsigned long long
+ht_slot_load(const unsigned long long *slots, uint32_t pos)
+{
+	return LDG ? __ldg(slots + pos) : slots[pos];
+}
+
+/* ExecScanHashBucket (nodeHash.c:2255) for an N:1 join: the walk from slot `pos`, whose entry `e` the caller loaded already
+ * (so that a caller can issue several rows' first loads together), to the first build row whose key equals the probe's.
+ * False when there is none, or when a key-in-slot table cannot hold the key at all. */
+template <bool LDG>
+__device__ __forceinline__ bool
+ht_find(const HtDev &ht, const unsigned long long *slots, uint32_t pos, unsigned long long e, uint32_t hash, const int64_t *key,
+		int nkeys, uint32_t *row)
+{
+	const uint32_t tag = ht_probe_tag(ht.keyslot, hash, key[0]);
+
+	if (ht.keyslot && !ht_key_in_domain(ht.keyslot, key[0]))
+		return false;
+	while (!ht_slot_empty(e))
+	{
+		if (ht_slot_match(ht, e, tag, key, nkeys))
+		{
+			*row = ht_slot_row(e);
+			return true;
+		}
+		pos = (pos + 1) & ht.mask;
+		e = ht_slot_load<LDG>(slots, pos);
+	}
+	return false;
+}
+#endif
 
 /* ---------------------------------------------------------------------------------------------
  * exact 128-bit accumulate built from 64-bit atomics.  Additions commute, so the final (hi, lo)

@@ -8,7 +8,8 @@
  * table is open addressing with linear probing over slots = hash32 << 32 | inner row id, at load
  * factor <= 0.5, and late-materialises: the inner payload stays in its column arrays and is
  * gathered by row id only for surviving rows.  The slot position uses the same 32-bit hash value
- * the reference computes (bucketno = hashvalue & (nbuckets - 1), nodeHash.c:2233).
+ * the reference computes (bucketno = hashvalue & (nbuckets - 1), nodeHash.c:2233).  The slot
+ * format and the N:1 walk live in common.cuh (ht_slot_entry .. ht_find), for every probing kernel.
  *
  * Probe restates ExecScanHashBucket (nodeHash.c:2255-2308): compare the stored hash value first,
  * then the key equality (hashqualclauses).
@@ -39,7 +40,7 @@ ht_row_hash(const HtDev &ht, uint32_t row, uint32_t *hash, int64_t *key0)
 
 		if (k == 0)
 			*key0 = v;
-		h = pg_hash_combine(h, jh_hash_datum(ht.keytype[k], v, ht.keydict[k]), false);
+		h = jh_key_fold(h, ht.keytype[k], v, ht.keydict[k]);
 	}
 	*hash = h;
 	return true;
@@ -85,7 +86,8 @@ k_ht_build(BuildParams p)
 			outside = true;		/* the host builds the table again with hash values in the slots */
 			v = false;
 		}
-		const unsigned long long e = ((unsigned long long) (p.ht.keyslot ? (uint32_t) key0 : h) << 32) | (uint32_t) i;
+		const uint32_t tag = ht_probe_tag(p.ht.keyslot, h, key0);
+		const unsigned long long e = ht_slot_entry(tag, (uint32_t) i);
 		uint32_t	pos = h & p.ht.mask;
 		const uint32_t bits = ht_bloom_bits(h, &w, p.ht.bloom_mask);
 
@@ -104,16 +106,15 @@ k_ht_build(BuildParams p)
 		{
 			unsigned long long c = cur;
 
-			if (c == HT_EMPTY)
+			if (ht_slot_empty(c))
 			{
 				c = atomicCAS(p.ht.slots + pos, HT_EMPTY, e);
-				if (c == HT_EMPTY)
+				if (ht_slot_empty(c))
 					break;
 			}
-			/* occupied: the same key -> a duplicate on the build side (key-in-slot tables see it in the slot; the others
+			/* occupied: the same key -> a duplicate on the build side (key-in-slot tables see it in the tag; the others
 			 * compare hash values first, then the keys by row id) */
-			if (!dup && (uint32_t) (c >> 32) == (uint32_t) (e >> 32) &&
-				(p.ht.keyslot || ht_keys_equal_rows(p.ht, (uint32_t) c, (uint32_t) e)))
+			if (!dup && ht_tag_match(c, tag) && (p.ht.keyslot || ht_keys_equal_rows(p.ht, ht_slot_row(c), (uint32_t) i)))
 				dup = true;
 			pos = (pos + 1) & p.ht.mask;
 			cur = p.ht.slots[pos];
@@ -426,7 +427,7 @@ ht_probe_row_batch(const ProbeParams &p, uint32_t row, int64_t *key, uint32_t *h
 		if (p.onulls[k] && p.onulls[k][row])
 			isnull = true;
 		key[k] = cb_load_widen(p.okey[k], p.otype[k], row);
-		h = pg_hash_combine(h, jh_hash_datum(p.otype[k], key[k], p.odict[k]), false);
+		h = jh_key_fold(h, p.otype[k], key[k], p.odict[k]);
 	}
 	*hash = h;
 	*keynull = isnull;
@@ -456,18 +457,6 @@ ht_probe_admits(const ProbeParams &p, uint32_t row, int64_t *key, uint32_t *h, b
 	return !isnull;
 }
 
-/* does slot entry e hold a build row whose key equals the outer row's (hash value first, then the key columns by row id)? */
-__device__ __forceinline__ bool
-ht_slot_key_equal(const ProbeParams &p, unsigned long long e, uint32_t h, const int64_t *key)
-{
-	if ((uint32_t) (e >> 32) != (p.ht.keyslot ? (uint32_t) key[0] : h))
-		return false;
-	for (int k = 0; k < p.ht.nkeys && !p.ht.keyslot; k++)
-		if (cb_load_widen(p.ht.keydata[k], p.ht.keytype[k], (uint32_t) e) != key[k])
-			return false;
-	return true;
-}
-
 template <bool WRITE>
 __global__ void __launch_bounds__(256)
 k_ht_probe_pairs(ProbeParams p)
@@ -486,23 +475,24 @@ k_ht_probe_pairs(ProbeParams p)
 
 		if (ht_probe_admits(p, row, key, &h, &mine))
 		{
+			const uint32_t tag = ht_probe_tag(p.ht.keyslot, h, key[0]);
 			uint32_t	pos = h & p.ht.mask;
 
 			for (;;)
 			{
 				unsigned long long e = p.ht.slots[pos];
 
-				if (e == HT_EMPTY)
+				if (ht_slot_empty(e))
 					break;
-				if (ht_slot_key_equal(p, e, h, key))
+				if (ht_slot_match(p.ht, e, tag, key, p.ht.nkeys))
 				{
 					if (WRITE)
 					{
 						p.out_outer[base + cnt] = row;
-						p.out_inner[base + cnt] = (uint32_t) e;
+						p.out_inner[base + cnt] = ht_slot_row(e);
 					}
 					else if (p.matched)
-						p.matched[(uint32_t) e] = 1;
+						p.matched[ht_slot_row(e)] = 1;
 					cnt++;
 				}
 				pos = (pos + 1) & p.ht.mask;
@@ -587,25 +577,26 @@ k_ht_probe_filtered(ProbeParams p)
 
 		if (ht_probe_admits(p, row, key, &h, &mine))
 		{
+			const uint32_t tag = ht_probe_tag(p.ht.keyslot, h, key[0]);
 			uint32_t	pos = h & p.ht.mask;
 
 			for (;;)
 			{
 				unsigned long long e = p.ht.slots[pos];
 
-				if (e == HT_EMPTY)
+				if (ht_slot_empty(e))
 					break;
-				if (ht_slot_key_equal(p, e, h, key) && join_filter_passes(p.f, row, (uint32_t) e))
+				if (ht_slot_match(p.ht, e, tag, key, p.ht.nkeys) && join_filter_passes(p.f, row, ht_slot_row(e)))
 				{
 					if (!left)
 					{
-						first = (uint32_t) e;
+						first = ht_slot_row(e);
 						break;
 					}
 					if (WRITE)
 					{
 						p.out_outer[base + cnt] = row;
-						p.out_inner[base + cnt] = (uint32_t) e;
+						p.out_inner[base + cnt] = ht_slot_row(e);
 					}
 					cnt++;
 				}

@@ -508,7 +508,7 @@ k_pipeline_generic(const __grid_constant__ PipeDev P)
 					}
 				}
 				for (int k = 0; k < pr.nkeys; k++)
-					h = pg_hash_combine(h, jh_hash_datum(pr.keytype[k], key[k], pr.keydict[k]), false);
+					h = jh_key_fold(h, pr.keytype[k], key[k], pr.keydict[k]);
 				if (knull && pr.null_key_drops)
 					alive = false;		/* NOT IN over a non-empty set: NULL <> everything is unknown, the row goes */
 				bool		maybe = alive && !knull;
@@ -534,19 +534,18 @@ k_pipeline_generic(const __grid_constant__ PipeDev P)
 					maybe = false;		/* outside the build side's key domain: no partner */
 				if (maybe)
 				{
+					/* ht_find's walk written out (through ht_find or ht_slot_match, ptxas gives this kernel more stack and spills) */
 					uint32_t	pos = h & pr.ht.mask;
+					unsigned long long e = pr.ht.slots[pos];
+					const uint32_t tag = ht_probe_tag(pr.ht.keyslot, h, key[0]);
 
-					for (;;)
+					while (!ht_slot_empty(e))
 					{
-						unsigned long long e = pr.ht.slots[pos];
-
-						if (e == HT_EMPTY)
-							break;
-						if ((uint32_t) (e >> 32) == (pr.ht.keyslot ? (uint32_t) key[0] : h))
+						if (ht_tag_match(e, tag))
 						{
 							bool		eq = true;
 
-							irow = (uint32_t) e;
+							irow = ht_slot_row(e);
 							for (int k = 0; k < pr.nkeys && !pr.ht.keyslot; k++)
 								if (cb_load_widen(pr.ht.keydata[k], pr.ht.keytype[k], irow) != key[k])
 									eq = false;
@@ -557,6 +556,7 @@ k_pipeline_generic(const __grid_constant__ PipeDev P)
 							}
 						}
 						pos = (pos + 1) & pr.ht.mask;
+						e = pr.ht.slots[pos];
 					}
 				}
 				/* join-type handling of the probe states (nodeHashjoin.c:583-713) */

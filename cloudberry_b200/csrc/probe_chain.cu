@@ -198,10 +198,10 @@ pc_key_hash(const PcProbe &pr, int64_t k0, int64_t k1)
 		return pg_hash_combine(0u, jh_mix32((uint32_t) (int32_t) k0), false);
 	if (KIND == 1)
 		return pg_hash_combine(0u, jh_int8(k0), false);
-	uint32_t	h = pg_hash_combine(0u, jh_hash_datum(pr.keytype[0], k0, pr.key[0].dict), false);
+	uint32_t	h = jh_key_fold(0u, pr.keytype[0], k0, pr.key[0].dict);
 
 	if (pr.nkeys > 1)
-		h = pg_hash_combine(h, jh_hash_datum(pr.keytype[1], k1, pr.key[1].dict), false);
+		h = jh_key_fold(h, pr.keytype[1], k1, pr.key[1].dict);
 	return h;
 }
 
@@ -219,6 +219,42 @@ pc_load_key0(const PcProbe &pr, uint32_t row, uint64_t pol_stream)
 	return cb_load_widen(pr.key[0].data, pr.key[0].type, row);
 }
 
+/* a stage's tail: the entries e[u] whose pass[u] is set go to the next queue in row order, as their j + 1 row ids and `word` as
+ * word j + 1 - one ballot per u (full-mask: every lane calls), one atomic per warp */
+__device__ __forceinline__ void
+pc_push(int j, const PcQ &Q, const uint32_t *e, const bool *pass, const uint32_t *word, uint32_t *out, unsigned ocap, unsigned *ocnt)
+{
+	const int	lane = threadIdx.x & 31;
+	uint32_t	bal[PC_U];
+	unsigned	tot = 0,
+				wb = 0;
+
+#pragma unroll
+	for (int u = 0; u < PC_U; u++)
+	{
+		bal[u] = __ballot_sync(0xffffffffu, pass[u]);
+		tot += __popc(bal[u]);
+	}
+	if (tot == 0)
+		return;
+	if (lane == 0)
+		wb = atomicAdd(ocnt, tot);
+	wb = __shfl_sync(0xffffffffu, wb, 0);
+#pragma unroll
+	for (int u = 0; u < PC_U; u++)
+	{
+		if ((bal[u] >> lane) & 1)
+		{
+			const uint32_t pos = wb + __popc(bal[u] & ((1u << lane) - 1));
+
+			for (int s = 0; s <= j; s++)
+				out[(size_t) s * ocap + pos] = pc_row(Q, s, e[u]);
+			out[(size_t) (j + 1) * ocap + pos] = word[u];
+		}
+		wb += __popc(bal[u]);
+	}
+}
+
 /* stage B_j: hash the join keys (ExecHashGetHashValue, nodeHash.c:2089) and test the build side's
  * Bloom filter.  in: entries [base, base + n) of Q (j + 1 row ids); out: the same row ids + hash. */
 template <int KIND>
@@ -229,10 +265,9 @@ pc_stage_bloom(const PcProbe &pr, int j, PcQ Q, unsigned base, unsigned n, uint3
 	const bool	use_bloom = pr.ht.bloom != NULL && pr.jointype != CB_JOIN_ANTI;
 	const uint64_t pol_stream = l2_policy_evict_first();
 	const uint64_t pol_keep = l2_policy_evict_last();
-	const int	lane = threadIdx.x & 31;
-	uint32_t	e[PC_U], h[PC_U], w[PC_U], bits[PC_U], word[PC_U], bal[PC_U];
+	uint32_t	e[PC_U], h[PC_U], w[PC_U], bits[PC_U], word[PC_U];
 	int64_t		k0[PC_U], k1[PC_U];
-	bool		v[PC_U];
+	bool		v[PC_U], pass[PC_U];
 
 #pragma unroll
 	for (int u = 0; u < PC_U; u++)
@@ -259,154 +294,27 @@ pc_stage_bloom(const PcProbe &pr, int j, PcQ Q, unsigned base, unsigned n, uint3
 		for (int u = 0; u < PC_U; u++)
 			word[u] = ldg_hint_u32(pr.ht.bloom + w[u], pol_keep);
 	}
-	/* one reservation per warp for all PC_U rows of every lane; entries stay in row order */
-	unsigned	tot = 0,
-				wb = 0;
-
 #pragma unroll
 	for (int u = 0; u < PC_U; u++)
-	{
-		const bool	pass = v[u] && (!use_bloom || (word[u] & bits[u]) == bits[u]);
-
-		bal[u] = __ballot_sync(0xffffffffu, pass);
-		tot += __popc(bal[u]);
-	}
-	if (tot == 0)
-		return;
-	if (lane == 0)
-		wb = atomicAdd(ocnt, tot);
-	wb = __shfl_sync(0xffffffffu, wb, 0);
-#pragma unroll
-	for (int u = 0; u < PC_U; u++)
-	{
-		if ((bal[u] >> lane) & 1)
-		{
-			const uint32_t pos = wb + __popc(bal[u] & ((1u << lane) - 1));
-
-			for (int s = 0; s <= j; s++)
-				out[(size_t) s * ocap + pos] = pc_row(Q, s, e[u]);
-			out[(size_t) (j + 1) * ocap + pos] = h[u];
-		}
-		wb += __popc(bal[u]);
-	}
+		pass[u] = v[u] && (!use_bloom || (word[u] & bits[u]) == bits[u]);
+	pc_push(j, Q, e, pass, h, out, ocap, ocnt);
 }
 
-/* stage H_j: ExecScanHashBucket (nodeHash.c:2255) for the rows that passed the filter: linear
- * probing from hash & mask, stored hash compared first, then the key itself.
- * in: j + 1 row ids + hash; out: j + 2 row ids. */
-template <int KIND>
+/* stage H_j / D_j: ExecScanHashBucket (nodeHash.c:2255) through ht_find, N:1.  in: j + 1 row ids; out: j + 2 row ids.
+ * FROM_QUEUE (stage H_j, after B_j): the key hash rides in the queue as word j + 1, slots are read through __ldg from HBM.
+ * Otherwise (stage D_j, PcProbe.mode 1 / 2) the stage hashes the keys itself and reads `slots`, the table in global memory
+ * or the CTA's copy in shared memory, with plain loads; its output goes to queue 2j + 2 (queue 2j + 1 stays empty).
+ * Every row's first slot load is issued before any is used. */
+template <int KIND, bool FROM_QUEUE>
 __device__ __noinline__ void
-pc_stage_ht(const PcProbe &pr, int j, PcQ Q, unsigned base, unsigned n, uint32_t *out, unsigned ocap, unsigned *ocnt)
+pc_stage_table(const PcProbe &pr, int j, PcQ Q, unsigned base, unsigned n, uint32_t *out, unsigned ocap, unsigned *ocnt,
+			   const unsigned long long *slots)
 {
 	const uint64_t pol_stream = l2_policy_evict_first();
-	const int	lane = threadIdx.x & 31;
-	uint32_t	e[PC_U], h[PC_U], pos[PC_U], irow[PC_U], bal[PC_U];
-	unsigned long long slot[PC_U];
-	bool		v[PC_U];
-
-#pragma unroll
-	for (int u = 0; u < PC_U; u++)
-	{
-		const unsigned i = u * PC_THREADS + threadIdx.x;
-
-		v[u] = i < n;
-		e[u] = base + (v[u] ? i : 0u);
-		h[u] = Q.q[(size_t) (j + 1) * Q.cap + e[u]];
-		pos[u] = h[u] & pr.ht.mask;
-	}
-#pragma unroll
-	for (int u = 0; u < PC_U; u++)
-		slot[u] = v[u] ? __ldg(pr.ht.slots + pos[u]) : HT_EMPTY;
-	unsigned	tot = 0,
-				wb = 0;
-
-#pragma unroll
-	for (int u = 0; u < PC_U; u++)
-	{
-		bool		found = false;
-
-		irow[u] = 0;
-		if (slot[u] != HT_EMPTY)
-		{
-			const int64_t k0 = pc_load_key0<KIND>(pr, pc_row(Q, pr.key[0].src, e[u]), pol_stream);
-			const int64_t k1 = (KIND == 2 && pr.nkeys > 1) ? pc_load(pr.key[1], Q, e[u]) : 0;
-			unsigned long long x = slot[u];
-			uint32_t	p = pos[u];
-
-			if (pr.ht.keyslot)
-			{
-				/* key-in-slot table: the slot settles it, no access to the build side's key column */
-				const uint32_t tag = (uint32_t) k0;
-
-				if (ht_key_in_domain(pr.ht.keyslot, k0))
-					while (x != HT_EMPTY)
-					{
-						if ((uint32_t) (x >> 32) == tag)
-						{
-							found = true;
-							irow[u] = (uint32_t) x;
-							break;
-						}
-						p = (p + 1) & pr.ht.mask;
-						x = __ldg(pr.ht.slots + p);
-					}
-			}
-			else
-				while (x != HT_EMPTY)
-				{
-					if ((uint32_t) (x >> 32) == h[u])
-					{
-						const uint32_t r = (uint32_t) x;
-
-						if (cb_load_widen(pr.ht.keydata[0], pr.ht.keytype[0], r) == k0 &&
-							(KIND != 2 || pr.nkeys < 2 || cb_load_widen(pr.ht.keydata[1], pr.ht.keytype[1], r) == k1))
-						{
-							found = true;
-							irow[u] = r;
-							break;
-						}
-					}
-					p = (p + 1) & pr.ht.mask;
-					x = __ldg(pr.ht.slots + p);
-				}
-		}
-		/* full-mask ballot: the warp reconverges here */
-		bal[u] = __ballot_sync(0xffffffffu, v[u] && (pr.jointype == CB_JOIN_ANTI ? !found : found));
-		tot += __popc(bal[u]);
-	}
-	if (tot == 0)
-		return;
-	if (lane == 0)
-		wb = atomicAdd(ocnt, tot);
-	wb = __shfl_sync(0xffffffffu, wb, 0);
-#pragma unroll
-	for (int u = 0; u < PC_U; u++)
-	{
-		if ((bal[u] >> lane) & 1)
-		{
-			const uint32_t opos = wb + __popc(bal[u] & ((1u << lane) - 1));
-
-			for (int s = 0; s <= j; s++)
-				out[(size_t) s * ocap + opos] = pc_row(Q, s, e[u]);
-			out[(size_t) (j + 1) * ocap + opos] = irow[u];
-		}
-		wb += __popc(bal[u]);
-	}
-}
-
-/* stage D_j (PcProbe.mode 1 / 2): key hash and table probe in one stage, for tables that stay in L2 (`slots` = the
- * table in global memory) or were staged into shared memory (`slots` = the CTA's copy).
- * in: j + 1 row ids; out: j + 2 row ids, into queue 2j + 2 (queue 2j + 1 stays empty). */
-template <int KIND>
-__device__ __noinline__ void
-pc_stage_direct(const PcProbe &pr, int j, PcQ Q, unsigned base, unsigned n, uint32_t *out, unsigned ocap, unsigned *ocnt, const unsigned long long *slots)
-{
-	const uint64_t pol_stream = l2_policy_evict_first();
-	const int	lane = threadIdx.x & 31;
-	uint32_t	e[PC_U], h[PC_U], pos[PC_U], irow[PC_U], bal[PC_U];
+	uint32_t	e[PC_U], h[PC_U], pos[PC_U], irow[PC_U];
 	int64_t		k0[PC_U], k1[PC_U];
 	unsigned long long slot[PC_U];
-	bool		v[PC_U];
+	bool		v[PC_U], pass[PC_U];
 
 #pragma unroll
 	for (int u = 0; u < PC_U; u++)
@@ -415,86 +323,47 @@ pc_stage_direct(const PcProbe &pr, int j, PcQ Q, unsigned base, unsigned n, uint
 
 		v[u] = i < n;
 		e[u] = base + (v[u] ? i : 0u);
-		k0[u] = pc_load_key0<KIND>(pr, pc_row(Q, pr.key[0].src, e[u]), pol_stream);
-		k1[u] = (KIND == 2 && pr.nkeys > 1) ? pc_load(pr.key[1], Q, e[u]) : 0;
+		if (FROM_QUEUE)
+			h[u] = Q.q[(size_t) (j + 1) * Q.cap + e[u]];
+		else
+		{
+			k0[u] = pc_load_key0<KIND>(pr, pc_row(Q, pr.key[0].src, e[u]), pol_stream);
+			k1[u] = (KIND == 2 && pr.nkeys > 1) ? pc_load(pr.key[1], Q, e[u]) : 0;
+		}
 	}
 #pragma unroll
 	for (int u = 0; u < PC_U; u++)
 	{
-		h[u] = pc_key_hash<KIND>(pr, k0[u], k1[u]);
+		if (!FROM_QUEUE)
+			h[u] = pc_key_hash<KIND>(pr, k0[u], k1[u]);
 		pos[u] = h[u] & pr.ht.mask;
 	}
 #pragma unroll
 	for (int u = 0; u < PC_U; u++)
-		slot[u] = v[u] ? slots[pos[u]] : HT_EMPTY;
-	unsigned	tot = 0,
-				wb = 0;
-
+		slot[u] = v[u] ? ht_slot_load<FROM_QUEUE>(slots, pos[u]) : HT_EMPTY;
 #pragma unroll
 	for (int u = 0; u < PC_U; u++)
 	{
 		bool		found = false;
-		unsigned long long x = slot[u];
-		uint32_t	p = pos[u];
 
 		irow[u] = 0;
-		if (pr.ht.keyslot)
+		if (!ht_slot_empty(slot[u]))
 		{
-			const uint32_t tag = (uint32_t) k0[u];
-
-			if (ht_key_in_domain(pr.ht.keyslot, k0[u]))
-				while (x != HT_EMPTY)
-				{
-					if ((uint32_t) (x >> 32) == tag)
-					{
-						found = true;
-						irow[u] = (uint32_t) x;
-						break;
-					}
-					p = (p + 1) & pr.ht.mask;
-					x = slots[p];
-				}
-		}
-		else
-			while (x != HT_EMPTY)
+			if (FROM_QUEUE)
 			{
-				if ((uint32_t) (x >> 32) == h[u])
-				{
-					const uint32_t r = (uint32_t) x;
-
-					if (cb_load_widen(pr.ht.keydata[0], pr.ht.keytype[0], r) == k0[u] &&
-						(KIND != 2 || pr.nkeys < 2 || cb_load_widen(pr.ht.keydata[1], pr.ht.keytype[1], r) == k1[u]))
-					{
-						found = true;
-						irow[u] = r;
-						break;
-					}
-				}
-				p = (p + 1) & pr.ht.mask;
-				x = slots[p];
+				/* stage H gathers the keys only of rows whose first slot is taken */
+				k0[u] = pc_load_key0<KIND>(pr, pc_row(Q, pr.key[0].src, e[u]), pol_stream);
+				k1[u] = (KIND == 2 && pr.nkeys > 1) ? pc_load(pr.key[1], Q, e[u]) : 0;
 			}
-		/* full-mask ballot: the warp reconverges here */
-		bal[u] = __ballot_sync(0xffffffffu, v[u] && (pr.jointype == CB_JOIN_ANTI ? !found : found));
-		tot += __popc(bal[u]);
-	}
-	if (tot == 0)
-		return;
-	if (lane == 0)
-		wb = atomicAdd(ocnt, tot);
-	wb = __shfl_sync(0xffffffffu, wb, 0);
-#pragma unroll
-	for (int u = 0; u < PC_U; u++)
-	{
-		if ((bal[u] >> lane) & 1)
-		{
-			const uint32_t opos = wb + __popc(bal[u] & ((1u << lane) - 1));
+			const int64_t key[2] = {k0[u], k1[u]};
+			uint32_t	r = 0;
 
-			for (int s = 0; s <= j; s++)
-				out[(size_t) s * ocap + opos] = pc_row(Q, s, e[u]);
-			out[(size_t) (j + 1) * ocap + opos] = irow[u];
+			found = ht_find<FROM_QUEUE>(pr.ht, slots, pos[u], slot[u], h[u], key, KIND == 2 ? pr.nkeys : 1, &r);
+			irow[u] = found ? r : 0;
 		}
-		wb += __popc(bal[u]);
+		pass[u] = v[u] && (pr.jointype == CB_JOIN_ANTI ? !found : found);
 	}
+	pc_push(j, Q, e, pass, irow, out, ocap, ocnt);
 }
 
 /* sink over entries [base, base + n) of the last queue (np + 1 row ids) */
@@ -752,6 +621,90 @@ pc_warp_dense(bool full, unsigned am, unsigned at_least = 64u)
 	return __all_sync(0xffffffffu, full) && __reduce_add_sync(0xffffffffu, (unsigned) __popc(am)) >= at_least;
 }
 
+/* where a thread's survivors among its 8 rows (bit u of am: row u) go in a queue whose fill count is *cnt: the warp's survivors
+ * stay in row order, with one warp scan and one atomic per warp.  Every lane calls. */
+__device__ __forceinline__ unsigned
+pc_compact8(unsigned am, unsigned *cnt)
+{
+	const int	lane = threadIdx.x & 31;
+	const unsigned c = __popc(am);
+	unsigned	x = c;
+
+#pragma unroll
+	for (int d = 1; d < 32; d <<= 1)
+	{
+		const unsigned y = __shfl_up_sync(0xffffffffu, x, d);
+
+		if (lane >= d)
+			x += y;
+	}
+	const unsigned total = __shfl_sync(0xffffffffu, x, 31);
+	unsigned	wb = 0;
+
+	if (lane == 31 && total)
+		wb = atomicAdd(cnt, total);
+	wb = __shfl_sync(0xffffffffu, wb, 31);
+	return wb + x - c;
+}
+
+/* ExecQual's range quals and the visimap over a thread's 8 rows o0 .. o0 + 7 of the tile at `base` (nvalid rows): the alive mask.
+ * A full 8 rows of a 4-byte qual column are two 16-byte loads, of a 1-byte column one 8-byte load, all issued before any is
+ * used; a partial tile loads row by row. */
+__device__ __forceinline__ unsigned
+pc_qual8(int32_t nfilters, const PcFilter *filt, const uint8_t *visimap, int64_t base, unsigned o0, unsigned nvalid, uint64_t pol_stream)
+{
+	unsigned	am = 0;
+
+	if (o0 + 8 <= nvalid)
+	{
+		int4		a0 = make_int4(0, 0, 0, 0), b0 = a0, a1 = a0, b1 = a0;
+		unsigned	vm = 0xff;
+
+		if (nfilters > 0)
+		{
+			if (filt[0].width == 4)
+			{
+				a0 = ldg_stream_v4((const int4 *) ((const int32_t *) filt[0].col + base + o0), pol_stream);
+				b0 = ldg_stream_v4((const int4 *) ((const int32_t *) filt[0].col + base + o0) + 1, pol_stream);
+			}
+			else
+				pc_unpack8(ldg_stream_u64((const unsigned long long *) ((const uint8_t *) filt[0].col + base + o0), pol_stream), &a0, &b0);
+		}
+		if (nfilters > 1)
+		{
+			if (filt[1].width == 4)
+			{
+				a1 = ldg_stream_v4((const int4 *) ((const int32_t *) filt[1].col + base + o0), pol_stream);
+				b1 = ldg_stream_v4((const int4 *) ((const int32_t *) filt[1].col + base + o0) + 1, pol_stream);
+			}
+			else
+				pc_unpack8(ldg_stream_u64((const unsigned long long *) ((const uint8_t *) filt[1].col + base + o0), pol_stream), &a1, &b1);
+		}
+		if (visimap)
+			vm = __ldg(visimap + ((base + o0) >> 3));
+		am = vm;
+		if (nfilters > 0)
+			am &= pc_range8(a0, b0, filt[0].lo, filt[0].span);
+		if (nfilters > 1)
+			am &= pc_range8(a1, b1, filt[1].lo, filt[1].span);
+	}
+	else
+		for (int u = 0; u < 8; u++)
+		{
+			const int64_t r = base + o0 + u;
+			bool		alive = o0 + u < nvalid;
+
+			if (alive && visimap)
+				alive = (__ldg(visimap + (r >> 3)) >> (r & 7)) & 1;
+			if (alive && nfilters > 0)
+				alive = (unsigned) (pc_filter_value(filt[0], r) - filt[0].lo) <= filt[0].span;
+			if (alive && nfilters > 1)
+				alive = (unsigned) (pc_filter_value(filt[1], r) - filt[1].lo) <= filt[1].span;
+			am |= (unsigned) alive << u;
+		}
+	return am;
+}
+
 /* stage F's tail when probe 0 is fused into it (P.fuse0): hash of the 8 keys, Bloom words of the alive ones in flight
  * together, survivors to queue 1 as (row id, hash) in row order - one warp scan, one shared-memory atomic.
  * WIDE: int8 key, else int4 / date. */
@@ -761,7 +714,6 @@ pc_stage_f_probe0(const PcProbe &pr, int64_t row0, const PcKeys8 &keys, unsigned
 {
 	const bool	use_bloom = pr.ht.bloom != NULL && pr.jointype != CB_JOIN_ANTI;
 	const uint64_t pol_keep = l2_policy_evict_last();
-	const int	lane = threadIdx.x & 31;
 	uint32_t	h[8];
 
 #pragma unroll
@@ -784,24 +736,7 @@ pc_stage_f_probe0(const PcProbe &pr, int64_t row0, const PcKeys8 &keys, unsigned
 			if ((word[u] & bits[u]) != bits[u])
 				am &= ~(1u << u);
 	}
-	const unsigned c = __popc(am);
-	unsigned	x = c;
-
-#pragma unroll
-	for (int d = 1; d < 32; d <<= 1)
-	{
-		const unsigned y = __shfl_up_sync(0xffffffffu, x, d);
-
-		if (lane >= d)
-			x += y;
-	}
-	const unsigned total = __shfl_sync(0xffffffffu, x, 31);
-	unsigned	wb = 0;
-
-	if (lane == 31 && total)
-		wb = atomicAdd(ocnt, total);
-	wb = __shfl_sync(0xffffffffu, wb, 31);
-	unsigned	pos = wb + x - c;
+	unsigned	pos = pc_compact8(am, ocnt);
 
 #pragma unroll
 	for (int u = 0; u < 8; u++)
@@ -813,31 +748,7 @@ pc_stage_f_probe0(const PcProbe &pr, int64_t row0, const PcKeys8 &keys, unsigned
 		}
 }
 
-/* a scan-level runtime filter over the thread's 8 rows: returns the alive mask with the rows that miss it cleared */
-template <bool WIDE>
-__device__ __forceinline__ unsigned
-pc_early_filter8(const PcEarly &E, int64_t row0, bool full, unsigned am, uint64_t pol)
-{
-	const PcKeys8 keys = pc_warp_dense(full, am) ? pc_keys8_vec<WIDE>(E.col, row0, pol) : pc_keys8_pred<WIDE>(E.col, row0, am, pol);
-	uint32_t	bits[8], word[8];
-
-#pragma unroll
-	for (int u = 0; u < 8; u++)
-	{
-		const int64_t kv = pc_keys8_get<WIDE>(keys, u);
-		uint32_t	w;
-
-		bits[u] = ht_bloom_bits(pg_hash_combine(0u, WIDE ? jh_int8(kv) : jh_mix32((uint32_t) (int32_t) kv), false), &w, E.mask);
-		word[u] = ((am >> u) & 1) ? __ldg(E.bloom + w) : 0u;
-	}
-#pragma unroll
-	for (int u = 0; u < 8; u++)
-		if ((word[u] & bits[u]) != bits[u])
-			am &= ~(1u << u);
-	return am;
-}
-
-/* the same test over keys that are in registers already */
+/* a scan-level runtime filter over 8 rows whose keys are in registers: the alive mask with the rows that miss it cleared */
 template <bool WIDE>
 __device__ __forceinline__ unsigned
 pc_bloom8_keys(const PcEarly &E, const PcKeys8 &keys, unsigned am)
@@ -858,6 +769,14 @@ pc_bloom8_keys(const PcEarly &E, const PcKeys8 &keys, unsigned am)
 		if ((word[u] & bits[u]) != bits[u])
 			am &= ~(1u << u);
 	return am;
+}
+
+/* the same test over the thread's 8 rows from row0 on: their keys loaded first */
+template <bool WIDE>
+__device__ __forceinline__ unsigned
+pc_early_filter8(const PcEarly &E, int64_t row0, bool full, unsigned am, uint64_t pol)
+{
+	return pc_bloom8_keys<WIDE>(E, pc_warp_dense(full, am) ? pc_keys8_vec<WIDE>(E.col, row0, pol) : pc_keys8_pred<WIDE>(E.col, row0, am, pol), am);
 }
 
 /* ---------------------------------------------------------------------------------------------
@@ -892,7 +811,6 @@ k_prefilter(const __grid_constant__ PfParams P)
 	__shared__ unsigned long long s_gbase;
 	const int64_t ntiles = (P.nrows + PC_TILE - 1) / PC_TILE;
 	const unsigned o0 = threadIdx.x * 8;
-	const int	lane = threadIdx.x & 31;
 	const uint64_t pol_stream = l2_policy_evict_first();
 
 	for (int64_t tile = blockIdx.x; tile < ntiles; tile += gridDim.x)
@@ -900,8 +818,7 @@ k_prefilter(const __grid_constant__ PfParams P)
 		const int64_t base = tile * PC_TILE;
 		const unsigned nvalid = (unsigned) (P.nrows - base < PC_TILE ? P.nrows - base : PC_TILE);
 		const bool	full = o0 + 8 <= nvalid;
-		unsigned	am = 0;
-
+		unsigned	am;
 		PcKeys8		keys0;
 		bool		have0 = false;
 
@@ -915,53 +832,7 @@ k_prefilter(const __grid_constant__ PfParams P)
 				: pc_keys8_vec<false>(P.bloom[0].col, base + o0, pol_stream);
 			have0 = true;
 		}
-		if (full)
-		{
-			int4		a0 = make_int4(0, 0, 0, 0), b0 = a0, a1 = a0, b1 = a0;
-			unsigned	vm = 0xff;
-
-			if (P.nfilters > 0)
-			{
-				if (P.filt[0].width == 4)
-				{
-					a0 = ldg_stream_v4((const int4 *) ((const int32_t *) P.filt[0].col + base + o0), pol_stream);
-					b0 = ldg_stream_v4((const int4 *) ((const int32_t *) P.filt[0].col + base + o0) + 1, pol_stream);
-				}
-				else
-					pc_unpack8(ldg_stream_u64((const unsigned long long *) ((const uint8_t *) P.filt[0].col + base + o0), pol_stream), &a0, &b0);
-			}
-			if (P.nfilters > 1)
-			{
-				if (P.filt[1].width == 4)
-				{
-					a1 = ldg_stream_v4((const int4 *) ((const int32_t *) P.filt[1].col + base + o0), pol_stream);
-					b1 = ldg_stream_v4((const int4 *) ((const int32_t *) P.filt[1].col + base + o0) + 1, pol_stream);
-				}
-				else
-					pc_unpack8(ldg_stream_u64((const unsigned long long *) ((const uint8_t *) P.filt[1].col + base + o0), pol_stream), &a1, &b1);
-			}
-			if (P.visimap)
-				vm = __ldg(P.visimap + ((base + o0) >> 3));
-			am = vm;
-			if (P.nfilters > 0)
-				am &= pc_range8(a0, b0, P.filt[0].lo, P.filt[0].span);
-			if (P.nfilters > 1)
-				am &= pc_range8(a1, b1, P.filt[1].lo, P.filt[1].span);
-		}
-		else
-			for (int u = 0; u < 8; u++)
-			{
-				const int64_t r = base + o0 + u;
-				bool		alive = o0 + u < nvalid;
-
-				if (alive && P.visimap)
-					alive = (__ldg(P.visimap + (r >> 3)) >> (r & 7)) & 1;
-				if (alive && P.nfilters > 0)
-					alive = (unsigned) (pc_filter_value(P.filt[0], r) - P.filt[0].lo) <= P.filt[0].span;
-				if (alive && P.nfilters > 1)
-					alive = (unsigned) (pc_filter_value(P.filt[1], r) - P.filt[1].lo) <= P.filt[1].span;
-				am |= (unsigned) alive << u;
-			}
+		am = pc_qual8(P.nfilters, P.filt, P.visimap, base, o0, nvalid, pol_stream);
 		for (int f = 0; f < P.nbloom && __any_sync(0xffffffffu, am != 0); f++)
 		{
 			if (SPEC && f == 0 && have0)
@@ -972,25 +843,8 @@ k_prefilter(const __grid_constant__ PfParams P)
 		}
 		__syncthreads();				/* s_cnt = 0 is in */
 		{
-			/* the tile's survivors, in row order within each warp: one scan + one shared atomic per warp */
-			const unsigned c = __popc(am);
-			unsigned	x = c;
-
-#pragma unroll
-			for (int d = 1; d < 32; d <<= 1)
-			{
-				const unsigned y = __shfl_up_sync(0xffffffffu, x, d);
-
-				if (lane >= d)
-					x += y;
-			}
-			const unsigned total = __shfl_sync(0xffffffffu, x, 31);
-			unsigned	wb = 0;
-
-			if (lane == 31 && total)
-				wb = atomicAdd(&s_cnt, total);
-			wb = __shfl_sync(0xffffffffu, wb, 31);
-			unsigned	pos = wb + x - c;
+			/* the tile's survivors, in row order within each warp */
+			unsigned	pos = pc_compact8(am, &s_cnt);
 
 #pragma unroll
 			for (int u = 0; u < 8; u++)
@@ -1107,60 +961,11 @@ k_probe_chain(const __grid_constant__ PcParams P)
 			const int64_t base = s_tile * PC_TILE;
 			const unsigned nvalid = (unsigned) (P.nrows - base < PC_TILE ? P.nrows - base : PC_TILE);
 			const unsigned o0 = threadIdx.x * 8;
-			const int	lane = threadIdx.x & 31;
 			const uint64_t pol_stream = l2_policy_evict_first();
 			const bool	full = o0 + 8 <= nvalid;
 			const bool	wide0 = sprobe[0].kind == 1;
-			unsigned	am = 0;
+			unsigned	am = pc_qual8(P.nfilters, P.filt, P.visimap, base, o0, nvalid, pol_stream);
 
-			if (full)
-			{
-				int4		a0 = make_int4(0, 0, 0, 0), b0 = a0, a1 = a0, b1 = a0;
-				unsigned	vm = 0xff;
-
-				/* 8 rows of a 4-byte column are two 16-byte loads, of a 1-byte column one 8-byte load */
-				if (P.nfilters > 0)
-				{
-					if (P.filt[0].width == 4)
-					{
-						a0 = ldg_stream_v4((const int4 *) ((const int32_t *) P.filt[0].col + base + o0), pol_stream);
-						b0 = ldg_stream_v4((const int4 *) ((const int32_t *) P.filt[0].col + base + o0) + 1, pol_stream);
-					}
-					else
-						pc_unpack8(ldg_stream_u64((const unsigned long long *) ((const uint8_t *) P.filt[0].col + base + o0), pol_stream), &a0, &b0);
-				}
-				if (P.nfilters > 1)
-				{
-					if (P.filt[1].width == 4)
-					{
-						a1 = ldg_stream_v4((const int4 *) ((const int32_t *) P.filt[1].col + base + o0), pol_stream);
-						b1 = ldg_stream_v4((const int4 *) ((const int32_t *) P.filt[1].col + base + o0) + 1, pol_stream);
-					}
-					else
-						pc_unpack8(ldg_stream_u64((const unsigned long long *) ((const uint8_t *) P.filt[1].col + base + o0), pol_stream), &a1, &b1);
-				}
-				if (P.visimap)
-					vm = __ldg(P.visimap + ((base + o0) >> 3));
-				am = vm;
-				if (P.nfilters > 0)
-					am &= pc_range8(a0, b0, P.filt[0].lo, P.filt[0].span);
-				if (P.nfilters > 1)
-					am &= pc_range8(a1, b1, P.filt[1].lo, P.filt[1].span);
-			}
-			else
-				for (int u = 0; u < 8; u++)
-				{
-					const int64_t r = base + o0 + u;
-					bool		alive = o0 + u < nvalid;
-
-					if (alive && P.visimap)
-						alive = (__ldg(P.visimap + (r >> 3)) >> (r & 7)) & 1;
-					if (alive && P.nfilters > 0)
-						alive = (unsigned) (pc_filter_value(P.filt[0], r) - P.filt[0].lo) <= P.filt[0].span;
-					if (alive && P.nfilters > 1)
-						alive = (unsigned) (pc_filter_value(P.filt[1], r) - P.filt[1].lo) <= P.filt[1].span;
-					am |= (unsigned) alive << u;
-				}
 			/* scan-level runtime filters: the key columns of the rows still alive, 8 filter words in flight */
 			for (int f = 0; f < P.nearly && __any_sync(0xffffffffu, am != 0); f++)
 				am = P.early[f].width == 8 ? pc_early_filter8<true>(P.early[f], base + o0, full, am, pol_stream)
@@ -1178,24 +983,7 @@ k_probe_chain(const __grid_constant__ PcParams P)
 											 qg + P.q_off[1], (unsigned) P.q_cap[1], &cnt[1]);
 				continue;
 			}
-			const unsigned c = __popc(am);
-			unsigned	x = c;
-
-#pragma unroll
-			for (int d = 1; d < 32; d <<= 1)
-			{
-				const unsigned y = __shfl_up_sync(0xffffffffu, x, d);
-
-				if (lane >= d)
-					x += y;
-			}
-			const unsigned total = __shfl_sync(0xffffffffu, x, 31);
-			unsigned	wb = 0;
-
-			if (lane == 31 && total)
-				wb = atomicAdd(&cnt[0], total);
-			wb = __shfl_sync(0xffffffffu, wb, 31);
-			unsigned	pos = wb + x - c;
+			unsigned	pos = pc_compact8(am, &cnt[0]);
 
 #pragma unroll
 			for (int u = 0; u < 8; u++)
@@ -1249,11 +1037,11 @@ k_probe_chain(const __grid_constant__ PcParams P)
 				uint32_t   *out2 = qg + P.q_off[s + 1];
 
 				if (pr.kind == 0)
-					pc_stage_direct<0>(pr, j, Q, base, n, out2, (unsigned) P.q_cap[s + 1], &cnt[s + 1], slots);
+					pc_stage_table<0, false>(pr, j, Q, base, n, out2, (unsigned) P.q_cap[s + 1], &cnt[s + 1], slots);
 				else if (pr.kind == 1)
-					pc_stage_direct<1>(pr, j, Q, base, n, out2, (unsigned) P.q_cap[s + 1], &cnt[s + 1], slots);
+					pc_stage_table<1, false>(pr, j, Q, base, n, out2, (unsigned) P.q_cap[s + 1], &cnt[s + 1], slots);
 				else
-					pc_stage_direct<2>(pr, j, Q, base, n, out2, (unsigned) P.q_cap[s + 1], &cnt[s + 1], slots);
+					pc_stage_table<2, false>(pr, j, Q, base, n, out2, (unsigned) P.q_cap[s + 1], &cnt[s + 1], slots);
 			}
 			else if (s & 1)
 			{
@@ -1267,11 +1055,11 @@ k_probe_chain(const __grid_constant__ PcParams P)
 			else
 			{
 				if (pr.kind == 0)
-					pc_stage_ht<0>(pr, j, Q, base, n, out, (unsigned) P.q_cap[s], &cnt[s]);
+					pc_stage_table<0, true>(pr, j, Q, base, n, out, (unsigned) P.q_cap[s], &cnt[s], pr.ht.slots);
 				else if (pr.kind == 1)
-					pc_stage_ht<1>(pr, j, Q, base, n, out, (unsigned) P.q_cap[s], &cnt[s]);
+					pc_stage_table<1, true>(pr, j, Q, base, n, out, (unsigned) P.q_cap[s], &cnt[s], pr.ht.slots);
 				else
-					pc_stage_ht<2>(pr, j, Q, base, n, out, (unsigned) P.q_cap[s], &cnt[s]);
+					pc_stage_table<2, true>(pr, j, Q, base, n, out, (unsigned) P.q_cap[s], &cnt[s], pr.ht.slots);
 			}
 		}
 	}
@@ -1325,36 +1113,17 @@ k_pc_early_build(PcEarlyBuild B)
 		{
 			const HtDev &T = B.red[m];
 			int64_t		kv[2] = {0, 0};
-			uint32_t	h = 0;
-			bool		found = false;
+			uint32_t	h = 0,
+						ir;
 
 			for (int i = 0; i < B.red_nkeys[m]; i++)
 			{
 				kv[i] = cb_load_widen(B.red_key[m][i].data, B.red_key[m][i].type, (uint32_t) r);
-				h = pg_hash_combine(h, jh_hash_datum(B.red_keytype[m][i], kv[i], B.red_key[m][i].dict), false);
+				h = jh_key_fold(h, B.red_keytype[m][i], kv[i], B.red_key[m][i].dict);
 			}
-			uint32_t	pos = h & T.mask;
+			const uint32_t pos = h & T.mask;
 
-			for (; !(T.keyslot && !ht_key_in_domain(T.keyslot, kv[0]));)
-			{
-				const unsigned long long e = T.slots[pos];
-
-				if (e == HT_EMPTY)
-					break;
-				if ((uint32_t) (e >> 32) == (T.keyslot ? (uint32_t) kv[0] : h))
-				{
-					const uint32_t ir = (uint32_t) e;
-
-					if (T.keyslot || (cb_load_widen(T.keydata[0], T.keytype[0], ir) == kv[0] &&
-									  (B.red_nkeys[m] < 2 || cb_load_widen(T.keydata[1], T.keytype[1], ir) == kv[1])))
-					{
-						found = true;
-						break;
-					}
-				}
-				pos = (pos + 1) & T.mask;
-			}
-			ok = found;
+			ok = ht_find<false>(T, T.slots, pos, T.slots[pos], h, kv, B.red_nkeys[m], &ir);
 		}
 		if (ok && !B.bloom)
 			atomicAdd(B.passed, 1ull);

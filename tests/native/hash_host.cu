@@ -1,7 +1,8 @@
 /* Host build of the hash functions the kernels inline (cloudberry_b200/csrc/common.cuh, the __host__ __device__ ones: the same
  * source text nvcc compiles into every join / aggregate / Motion kernel).  Test harness only: compiled by
  * tests/test_device_hash_source.py with nvcc (host side of the translation unit) and compared with the reference's own
- * hashfunc.c / varchar.c / cdbhash.c / hashfn.h as compiled into oracle/_ref/libexec_ref.so. */
+ * hashfunc.c / varchar.c / cdbhash.c / hashfn.h as compiled into oracle/_ref/libexec_ref.so.  The join table's slot format
+ * helpers (ht_*) are the same kind of source and are tested here too. */
 #include "../../cloudberry_b200/csrc/common.cuh"
 
 extern "C" {
@@ -13,4 +14,12 @@ uint32_t	hh_hash_bytes(const unsigned char *k, int len) { return pg_hash_bytes_h
 uint32_t	hh_murmurhash32(uint32_t h) { return pg_murmurhash32(h); }
 uint32_t	hh_hash_combine(uint32_t acc, uint32_t h, int isnull) { return pg_hash_combine(acc, h, isnull != 0); }
 int32_t		hh_jump_consistent_hash(uint64_t key, int32_t nseg) { return pg_jump_consistent_hash(key, nseg); }
+uint32_t	hh_jh_int8(int64_t v) { return jh_int8(v); }
+uint32_t	hh_jh_mix32(uint32_t x) { return jh_mix32(x); }
+int			hh_key_in_domain(int32_t keyslot, int64_t key) { return ht_key_in_domain(keyslot, key); }
+uint32_t	hh_probe_tag(int32_t keyslot, uint32_t hash, int64_t key0) { return ht_probe_tag(keyslot, hash, key0); }
+uint64_t	hh_slot_entry(uint32_t tag, uint32_t row) { return ht_slot_entry(tag, row); }
+int			hh_slot_empty(uint64_t e) { return ht_slot_empty(e); }
+uint32_t	hh_slot_row(uint64_t e) { return ht_slot_row(e); }
+int			hh_tag_match(uint64_t e, uint32_t tag) { return ht_tag_match(e, tag); }
 }

@@ -2,7 +2,9 @@
 and held against the reference's own code (not gpu): hashint4 / hashint8 / hashfloat8 / hashbpchar, murmurhash32, the
 rotate-xor key combination of nodeHash.c / execGrouping.c / cdbhash.c, and jump_consistent_hash through cdbhashreduce.
 On the device the same text runs with __ddiv_rn / __dmul_rn in the jump hash (IEEE, no contraction), which
-tests/test_gpu_multirank.py and the Motion tests check against the oracle's routes."""
+tests/test_gpu_multirank.py and the Motion tests check against the oracle's routes.  The join table's slot format (ht_slot_entry,
+ht_probe_tag, ht_tag_match, ht_key_in_domain) is the same kind of source and is held against its rule over the key sets
+tests/test_gpu_join_routes.py joins on."""
 import ctypes as C
 import os
 import random
@@ -33,6 +35,13 @@ def host(tmp_path_factory):
         getattr(H, name).argtypes = args
     H.hh_jump_consistent_hash.restype = C.c_int32
     H.hh_jump_consistent_hash.argtypes = [C.c_uint64, C.c_int32]
+    for name, res, args in (("hh_jh_int8", C.c_uint32, [C.c_int64]), ("hh_jh_mix32", C.c_uint32, [C.c_uint32]),
+                            ("hh_key_in_domain", C.c_int, [C.c_int32, C.c_int64]),
+                            ("hh_probe_tag", C.c_uint32, [C.c_int32, C.c_uint32, C.c_int64]),
+                            ("hh_slot_entry", C.c_uint64, [C.c_uint32, C.c_uint32]), ("hh_slot_empty", C.c_int, [C.c_uint64]),
+                            ("hh_slot_row", C.c_uint32, [C.c_uint64]), ("hh_tag_match", C.c_int, [C.c_uint64, C.c_uint32])):
+        getattr(H, name).restype = res
+        getattr(H, name).argtypes = args
     return H
 
 
@@ -129,3 +138,37 @@ def test_murmur_and_key_combination(libs):
         assert want >= 0
         assert H.hh_jump_consistent_hash(acc, nseg) == want, (ks, vals, nulls, nseg)
         assert R.ref_jump_consistent_hash(acc, nseg) == want
+
+
+def test_join_slot_format(host):
+    """a slot's tag and row round-trip, a probe's tag matches the tag its key was built with, and a key-in-slot table (keyslot 1:
+    int32 domain, 2: [0, 2^32)) never confuses two keys: inside its domain distinct keys have distinct tags, and a key outside
+    it is refused.  Key sets of tests/test_gpu_join_routes.py: int8 keys that share their low 32 bits or their hash fold, int4
+    at its limits, int8 keys just outside [0, 2^32)."""
+    H = host
+    i32min, i32max = -2 ** 31, 2 ** 31 - 1
+    rng = random.Random(79)
+    int8_keys = [0, 1, 7, 2 ** 32 - 1, 2 ** 32, 2 ** 32 + 7, 7 - 2 ** 32, -1, -2 ** 32, 2 ** 33 - 1, 2 ** 40 + 3, -5,
+                 i32min, i32max] + [rng.getrandbits(32) for _ in range(2000)] + [rng.getrandbits(40) for _ in range(500)]
+    int8_keys += [k + 2 ** 32 for k in int8_keys[:200]] + [k - 2 ** 32 for k in int8_keys[:200]]
+    fold = {}
+    for k in int8_keys:                                  # keys whose hashint8 fold (lo ^ hi, or lo ^ ~hi) agrees
+        lo, hi = k & 0xFFFFFFFF, (k >> 32) & 0xFFFFFFFF
+        fold.setdefault(lo ^ (hi if k >= 0 else ~hi & 0xFFFFFFFF), []).append(k)
+    assert any(len(set(v)) > 1 for v in fold.values())
+    int4_keys = [i32min, i32max, i32min + 1, i32max - 1, -1, 0, 1] + [rng.getrandbits(32) - 2 ** 31 for _ in range(2000)]
+    assert H.hh_slot_empty(0xFFFFFFFFFFFFFFFF) and not H.hh_slot_empty(0)
+    for keyslot, keys in ((2, int8_keys), (1, int4_keys), (1, int8_keys)):
+        tags = {}
+        for row, k in enumerate(set(keys)):
+            h = H.hh_jh_int8(k) if keys is int8_keys else H.hh_jh_mix32(k & 0xFFFFFFFF)
+            inside = H.hh_key_in_domain(keyslot, k)
+            assert inside == ((i32min <= k <= i32max) if keyslot == 1 else (0 <= k < 2 ** 32)), (keyslot, k)
+            for ks in (keyslot, 0):
+                tag = H.hh_probe_tag(ks, h, k)
+                e = H.hh_slot_entry(tag, row)
+                assert not H.hh_slot_empty(e) and H.hh_slot_row(e) == row and H.hh_tag_match(e, tag)
+                assert tag == (h if ks == 0 else k & 0xFFFFFFFF)
+            if inside:
+                tag = H.hh_probe_tag(keyslot, h, k)
+                assert tags.setdefault(tag, k) == k, (keyslot, k, tags[tag])
