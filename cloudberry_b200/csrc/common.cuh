@@ -638,8 +638,8 @@ pg_jump_consistent_hash(uint64_t key, int32_t num_segments)
 }
 
 /* hash function of one key datum by type (pg_amproc: hashint4, hashint8, hashfloat8, hashbpchar,
- * hashchar for bool) on the 64-bit widened value */
-__device__ __forceinline__ uint32_t
+ * hashchar for bool) on the 64-bit widened value; a dictionary code's hash is its entry of the per-code table */
+CB_HD uint32_t
 pg_hash_datum(int type, int64_t v, const uint32_t *dict)
 {
 	switch (type)
@@ -653,12 +653,93 @@ pg_hash_datum(int type, int64_t v, const uint32_t *dict)
 		case CB_BPCHAR1:
 			return pg_hash_bpchar1((uint8_t) v);
 		case CB_DICT8: case CB_DICT32:
+#ifdef __CUDA_ARCH__
 			return dict ? __ldg(dict + v) : 0u;
+#else
+			return dict ? dict[v] : 0u;
+#endif
 		case CB_BOOL:
 			return pg_hash_uint32((uint32_t) (int32_t) (int8_t) v);
 		default:
 			return 0u;
 	}
+}
+
+/* The hash compositions whose values are observable, written once for every sink (DESIGN §2).  Key k has type types[k],
+ * per-code hash table dicts[k] and value keys[k]; bit k of knull marks it NULL.  pg_hash_keys is the rotate-xor over the
+ * keys that the group hash and cdbhash share (a NULL contributes nothing). */
+CB_HD uint32_t
+pg_hash_keys(int nkeys, const int32_t *types, const uint32_t *const *dicts, const int64_t *keys, uint32_t knull)
+{
+	uint32_t	h = 0;
+
+	for (int k = 0; k < nkeys; k++)
+	{
+		const bool	isn = (knull >> k) & 1;
+
+		h = pg_hash_combine(h, isn ? 0u : pg_hash_datum(types[k], keys[k], dicts[k]), isn);
+	}
+	return h;
+}
+
+/* float8eq groups -0 with +0 and all NaNs together (hashfloat8 gives them one hash value, hashfunc.c:194-216); the
+ * aggregate table compares key bits, so a group key is made canonical first */
+CB_HD int64_t
+agg_group_key(int type, int64_t v)
+{
+	if (type == CB_FLOAT8 && ((uint64_t) v << 1) == 0)
+		return 0;
+	if (type == CB_FLOAT8 && ((v >> 52) & 0x7ff) == 0x7ff && (v & 0xfffffffffffffll) != 0)
+		return 0x7FF8000000000000ll;
+	return v;
+}
+
+/* TupleHashTableHash_internal (executor/execGrouping.c:437-495): hash_iv 0, rotate-xor per key, then murmurhash32 */
+CB_HD uint32_t
+agg_group_hash(int nkeys, const int32_t *types, const uint32_t *const *dicts, const int64_t *keys, uint32_t knull)
+{
+	return pg_murmurhash32(pg_hash_keys(nkeys, types, dicts, keys, knull));
+}
+
+/* the Motion's destination of a row: cdbhashinit / cdbhash / cdbhashreduce (cdb/cdbhash.c:171,189,253) */
+CB_HD int32_t
+cdb_route(int nkeys, const int32_t *types, const uint32_t *const *dicts, const int64_t *keys, uint32_t knull, int32_t nsegs)
+{
+	return pg_jump_consistent_hash(pg_hash_keys(nkeys, types, dicts, keys, knull), nsegs);
+}
+
+/* int8pl / int8mi / int8mul (utils/adt/int8.c) raise "bigint out of range"; the kernels refuse such a row, and scaled
+ * numerics share the check (a product that leaves 64 bits is refused, never wrapped).  Each returns the wrapped result
+ * and sets *ovf when the exact one does not fit. */
+CB_HD int64_t
+i64_add_ovf(int64_t x, int64_t y, bool *ovf)
+{
+	const int64_t r = (int64_t) ((uint64_t) x + (uint64_t) y);
+
+	*ovf = ((x ^ r) & (y ^ r)) < 0;
+	return r;
+}
+
+CB_HD int64_t
+i64_sub_ovf(int64_t x, int64_t y, bool *ovf)
+{
+	const int64_t r = (int64_t) ((uint64_t) x - (uint64_t) y);
+
+	*ovf = ((x ^ y) & (x ^ r)) < 0;
+	return r;
+}
+
+CB_HD int64_t
+i64_mul_ovf(int64_t x, int64_t y, bool *ovf)
+{
+	const int64_t r = (int64_t) ((uint64_t) x * (uint64_t) y);
+
+#ifdef __CUDA_ARCH__
+	*ovf = __mul64hi(x, y) != (r >> 63);
+#else
+	*ovf = (int64_t) (((__int128) x * y) >> 64) != (r >> 63);
+#endif
+	return r;
 }
 
 /* ---------------------------------------------------------------------------------------------

@@ -89,6 +89,7 @@ cb_pipeline_to_dev(cbgpu_ctx *ctx, const CbPipeline *p, PipeDev *d, XProg *xp)
 	}
 	const CbpSink *s = &p->sink;
 	DSink	   *ds = &d->sink;
+	SinkOut    *o = &ds->out;
 
 	ds->kind = s->kind;
 	switch (s->kind)
@@ -128,40 +129,39 @@ cb_pipeline_to_dev(cbgpu_ctx *ctx, const CbPipeline *p, PipeDev *d, XProg *xp)
 		case CBP_SINK_PARTITION:
 			if (!s->out || s->nout != xp->depth || s->nout > CBP_MAX_OUT || s->nout > s->out->ncols || !s->out_count)
 				return cb_fail(ctx, CBGPU_ERR_INVALID, "pipeline sink: output shape mismatch%s (%lld values)", "", xp->depth);
-			ds->nout = s->nout;
+			o->nout = s->nout;
 			for (int c = 0; c < s->nout; c++)
 			{
-				ds->outcol[c] = s->out->data[c];
-				ds->outnull[c] = s->out->nulls[c];
-				ds->outtype[c] = s->out->types[c];
+				o->outcol[c] = s->out->data[c];
+				o->outnull[c] = s->out->nulls[c];
+				o->outtype[c] = s->out->types[c];
 			}
-			ds->out_count = (unsigned long long *) s->out_count;
-			ds->out_capacity = s->out->capacity;
+			o->out_count = (unsigned long long *) s->out_count;
+			o->seg_cap[0] = s->out->capacity;
 			if (s->kind == CBP_SINK_PARTITION)
 			{
 				if (s->nsegs < 1 || s->nsegs > 64 || s->nhash < 1 || s->nhash > CBP_MAX_KEYS || s->nhash > s->nout ||
 					(!s->part_cols && !s->seg_base && s->seg_capacity * s->nsegs > s->out->capacity) || (s->part_cols && !s->part_counts) ||
 					(s->part_cols && s->part_nullmask && !s->part_nulls) || (!s->seg_base != !s->seg_cap))
 					return cb_fail(ctx, CBGPU_ERR_INVALID, "pipeline sink: bad partition description%s", "", 0);
-				ds->part_cols = s->part_cols;
-				ds->part_counts = s->part_counts;
-				ds->part_nulls = s->part_nulls;
-				ds->part_nullmask = s->part_cols ? s->part_nullmask : 0;
-				ds->part_flags = s->part_flags;
-				ds->nhash = s->nhash;
-				ds->nsegs = s->nsegs;
-				ds->seg_capacity = s->seg_capacity;
+				o->part_cols = s->part_cols;
+				o->part_counts = s->part_counts;
+				o->part_nulls = s->part_nulls;
+				o->part_nullmask = s->part_cols ? s->part_nullmask : 0;
+				o->part_flags = s->part_flags;
+				o->nhash = s->nhash;
+				o->nsegs = s->nsegs;
 				for (int g = 0; g < s->nsegs; g++)
 				{
-					ds->seg_base[g] = s->seg_base ? s->seg_base[g] : (int64_t) g * s->seg_capacity;
-					ds->seg_cap[g] = s->part_cols ? s->seg_capacity : s->seg_cap ? s->seg_cap[g] : s->seg_capacity;
-					if (!s->part_cols && (ds->seg_base[g] < 0 || ds->seg_cap[g] < 0 || ds->seg_base[g] + ds->seg_cap[g] > s->out->capacity))
+					o->seg_base[g] = s->seg_base ? s->seg_base[g] : (int64_t) g * s->seg_capacity;
+					o->seg_cap[g] = s->part_cols ? s->seg_capacity : s->seg_cap ? s->seg_cap[g] : s->seg_capacity;
+					if (!s->part_cols && (o->seg_base[g] < 0 || o->seg_cap[g] < 0 || o->seg_base[g] + o->seg_cap[g] > s->out->capacity))
 						return cb_fail(ctx, CBGPU_ERR_INVALID, "pipeline sink: destination %s%lld's range lies outside the send buffer", "", g);
 				}
 				for (int k = 0; k < s->nhash; k++)
 				{
-					ds->hashtype[k] = s->hashtype[k];
-					ds->hashdict[k] = s->hash_dict_hash[k];
+					o->hashtype[k] = s->hashtype[k];
+					o->hashdict[k] = s->hash_dict_hash[k];
 				}
 			}
 			break;
@@ -461,12 +461,11 @@ k_pipeline_generic(const __grid_constant__ PipeDev P)
 							bn;
 				int64_t		x = gen_load_col(P, a & 0xffff, ridx, rnull, alive, &an);
 				int64_t		b = gen_load_col(P, a >> 16, ridx, rnull, alive, &bn);
-				int64_t		k = P.ops[pc].imm;
-				int64_t		d = (int64_t) ((uint64_t) k - (uint64_t) b);
-				int64_t		r = (int64_t) ((uint64_t) x * (uint64_t) d);
-				bool		ovf = (((k ^ b) & (k ^ d)) < 0) || (__mul64hi(x, d) != (r >> 63));
+				bool		ovf_sub,
+							ovf_mul;
+				const int64_t r = i64_mul_ovf(x, i64_sub_ovf(P.ops[pc].imm, b, &ovf_sub), &ovf_mul);
 
-				if (alive && !an && !bn && ovf)
+				if (alive && !an && !bn && (ovf_sub || ovf_mul))
 					atomicExch(P.status, CBGPU_ERR_OVERFLOW);
 				st[sp] = r;
 				snull = (an || bn) ? (snull | (1ull << sp)) : (snull & ~(1ull << sp));
@@ -649,31 +648,12 @@ k_pipeline_generic(const __grid_constant__ PipeDev P)
 		{
 			if (alive)
 			{
-				/* TupleHashTableHash_internal (executor/execGrouping.c:437-495): hash_iv 0,
-				 * rotate-xor per key (NULL -> 0), then murmurhash32 */
-				uint32_t	h = 0;
-				uint32_t	knull = (uint32_t) (snull & ((1ull << S.nkeys) - 1));
+				const uint32_t knull = (uint32_t) (snull & ((1ull << S.nkeys) - 1));
 
 				for (int k = 0; k < S.nkeys; k++)
-				{
-					bool		isn = (knull >> k) & 1;
+					st[k] = ((knull >> k) & 1) ? 0 : agg_group_key(S.keytype[k], st[k]);
+				const uint32_t h = agg_group_hash(S.nkeys, S.keytype, S.keydict, st, knull);
 
-					if (isn)
-						st[k] = 0;
-					else if (S.keytype[k] == CB_FLOAT8)
-					{
-						/* float8eq groups -0 with +0 and all NaNs together (hashfloat8 gives them one hash value,
-						 * hashfunc.c:194-216); the table compares key bits, so the key is made canonical first */
-						const double dv = __longlong_as_double(st[k]);
-
-						if (dv == 0.0)
-							st[k] = 0;
-						else if (dv != dv)
-							st[k] = 0x7FF8000000000000ll;
-					}
-					h = pg_hash_combine(h, isn ? 0u : pg_hash_datum(S.keytype[k], st[k], S.keydict[k]), isn);
-				}
-				h = pg_murmurhash32(h);
 				/* partitioned aggregation: this pass owns the groups whose hash carries its number */
 				int			slot = (S.agg.npart > 1 && (int32_t) (h >> S.agg.part_shift) != S.agg.part_id) ? -1 : agg_find_or_insert(S.agg, h, st, knull);
 
@@ -686,72 +666,20 @@ k_pipeline_generic(const __grid_constant__ PipeDev P)
 		{
 			/* one output position per surviving row; positions handed out per warp and per
 			 * destination so the counters see one atomic per (warp, destination) */
-			int			seg = 0;
-
-			if (S.kind == CBP_SINK_PARTITION && alive)
-			{
-				/* cdbhashinit / cdbhash / cdbhashreduce (cdb/cdbhash.c:171,189,253) */
-				uint32_t	h = 0;
-
-				for (int k = 0; k < S.nhash; k++)
-				{
-					bool		isn = (snull >> k) & 1;
-
-					h = pg_hash_combine(h, isn ? 0u : pg_hash_datum(S.hashtype[k], st[k], S.hashdict[k]), isn);
-				}
-				seg = pg_jump_consistent_hash(h, S.nsegs);
-			}
-			uint32_t	amask = __ballot_sync(0xffffffffu, alive);
+			const SinkOut &O = S.out;
+			const int	seg = S.kind == CBP_SINK_PARTITION && alive ? cdb_route(O.nhash, O.hashtype, O.hashdict, st, (uint32_t) snull, O.nsegs) : 0;
+			const uint32_t amask = __ballot_sync(0xffffffffu, alive);
 
 			if (alive)
 			{
-				uint32_t	peers = __match_any_sync(amask, seg);
-				int			leader = __ffs(peers) - 1;
+				const uint32_t peers = __match_any_sync(amask, seg);
+				const int	leader = __ffs(peers) - 1;
 				unsigned long long pos = 0;
 
-				const bool	direct = S.kind == CBP_SINK_PARTITION && S.part_cols != NULL;
-
 				if (lane == leader)
-				{
-					pos = atomicAdd(S.out_count + seg, (unsigned long long) __popc(peers));
-					if (direct)		/* the slice of the DESTINATION's buffer; the local count stays as a statistic */
-						pos = atomicAdd_system(S.part_counts[seg], (unsigned long long) __popc(peers));
-				}
+					pos = sink_reserve(O, seg, __popc(peers), P.status);
 				pos = __shfl_sync(peers, pos, leader) + __popc(peers & ((1u << lane) - 1));
-				int64_t		cap = S.kind == CBP_SINK_PARTITION ? S.seg_cap[seg] : S.out_capacity;
-
-				if ((int64_t) pos >= cap)
-				{
-					/* a full Motion destination is not an error: the host redoes the pass with exact sizes */
-					if (S.kind == CBP_SINK_PARTITION && S.part_flags)
-						atomicOr(S.part_flags, CBGPU_DX_OVERFLOW);
-					else
-						atomicExch(P.status, CBGPU_ERR_NOMEM);
-				}
-				else if (direct)
-				{
-					for (int c = 0; c < S.nout; c++)
-					{
-						sink_store(S.part_cols[seg * S.nout + c], S.outtype[c], pos, st[c]);
-						if ((S.part_nullmask >> c) & 1)
-							S.part_nulls[seg * S.nout + c][pos] = (snull >> c) & 1;
-						else if ((snull >> c) & 1)
-							atomicExch(P.status, CBGPU_ERR_INVALID);
-					}
-				}
-				else
-				{
-					uint64_t	dst = (uint64_t) (S.kind == CBP_SINK_PARTITION ? S.seg_base[seg] : 0) + pos;
-
-					for (int c = 0; c < S.nout; c++)
-					{
-						sink_store(S.outcol[c], S.outtype[c], dst, st[c]);
-						if (S.outnull[c])
-							S.outnull[c][dst] = (snull >> c) & 1;
-						else if ((snull >> c) & 1)
-							atomicExch(P.status, CBGPU_ERR_INVALID);
-					}
-				}
+				sink_put_row(O, seg, pos, [&](int c) { return st[c]; }, snull, P.status);
 			}
 		}
 	}

@@ -22,6 +22,30 @@ struct DProbe
 	int32_t		null_key_drops;
 };
 
+/* Where the rows of a MATERIALIZE or PARTITION sink go, filled once by cb_pipeline_to_dev.  Destination d takes rows at
+ * positions [0, seg_cap[d]): in a direct Motion at those positions of the destination's own window (part_*), otherwise at
+ * seg_base[d] + position of the output columns.  MATERIALIZE is destination 0 with seg_base 0 and the output's capacity. */
+struct SinkOut
+{
+	int32_t		nout;
+	void	   *outcol[CBP_MAX_OUT];
+	uint8_t    *outnull[CBP_MAX_OUT];
+	int32_t		outtype[CBP_MAX_OUT];
+	unsigned long long *out_count;	/* per destination: every row routed there, stored or not            */
+	/* PARTITION: cdb_route over the first nhash output columns picks the destination */
+	int32_t		nhash;
+	int32_t		hashtype[CBP_MAX_KEYS];
+	const uint32_t *hashdict[CBP_MAX_KEYS];
+	int32_t		nsegs;
+	void *const *part_cols;		/* direct Motion: destination d's column c at part_cols[d * nout + c]  */
+	unsigned long long *const *part_counts;	/* ... and its row counter (peer memory)               */
+	uint8_t *const *part_nulls;	/* ... and its NULL bytes, for the columns in part_nullmask           */
+	unsigned long long part_nullmask;
+	int32_t    *part_flags;		/* a full destination ORs CBGPU_DX_OVERFLOW in here (NULL: status word) */
+	int64_t		seg_base[64];
+	int64_t		seg_cap[64];
+};
+
 struct DSink
 {
 	int32_t		kind;
@@ -31,24 +55,7 @@ struct DSink
 	const uint32_t *keydict[CBP_MAX_KEYS];
 	int32_t		naccs;
 	CbpAcc		accs[CBP_MAX_AGGS];
-	int32_t		nout;
-	void	   *outcol[CBP_MAX_OUT];
-	uint8_t    *outnull[CBP_MAX_OUT];
-	int32_t		outtype[CBP_MAX_OUT];
-	unsigned long long *out_count;
-	int64_t		out_capacity;
-	int32_t		nhash;
-	int32_t		hashtype[CBP_MAX_KEYS];
-	const uint32_t *hashdict[CBP_MAX_KEYS];
-	int32_t		nsegs;
-	int64_t		seg_capacity;
-	void *const *part_cols;		/* direct Motion: destination d's column c at part_cols[d * nout + c]  */
-	unsigned long long *const *part_counts;	/* ... and its row counter (peer memory)               */
-	uint8_t *const *part_nulls;	/* ... and its NULL bytes                                             */
-	unsigned long long part_nullmask;
-	int32_t    *part_flags;		/* a full destination ORs CBGPU_DX_OVERFLOW in here (NULL: status word) */
-	int64_t		seg_base[64];	/* staged: first row of destination d's range in the output columns    */
-	int64_t		seg_cap[64];	/* ... and how many rows fit                                           */
+	SinkOut		out;
 };
 
 struct PipeDev
@@ -163,8 +170,7 @@ fcmp_pg(double x, double y)
 /* One scalar op of a postfix program over the value stack st[0 .. sp) with NULL bits snull: CONST, DUP, POP, integer and float8
  * arithmetic, I2F, F8ORD, the compares and three-valued AND / OR / NOT.  The pipeline kernel and the join-filter probe both
  * run their programs through it; each reads columns (LOAD) and consumes results (FILTER) itself.  Integer overflow of a live
- * row (`alive`, operands not NULL) stores CBGPU_ERR_OVERFLOW in *status (int8pl / int8mi / int8mul report "bigint out of
- * range", utils/adt/int8.c). */
+ * row (`alive`, operands not NULL) stores CBGPU_ERR_OVERFLOW in *status (i64_add_ovf and its siblings). */
 __device__ __forceinline__ void
 cbp_scalar_op(const CbpOp &op, int64_t *st, uint64_t &snull, int &sp, bool alive, int *status)
 {
@@ -191,25 +197,9 @@ cbp_scalar_op(const CbpOp &op, int64_t *st, uint64_t &snull, int &sp, bool alive
 				int64_t		y = st[sp - 1],
 							x = st[sp - 2];
 				bool		n = ((snull >> (sp - 1)) | (snull >> (sp - 2))) & 1;
-				int64_t		r;
 				bool		ovf;
+				const int64_t r = code == CBP_ADD ? i64_add_ovf(x, y, &ovf) : code == CBP_SUB ? i64_sub_ovf(x, y, &ovf) : i64_mul_ovf(x, y, &ovf);
 
-				/* scaled numerics share the check: a product that leaves 64 bits is refused, never wrapped */
-				if (code == CBP_ADD)
-				{
-					r = (int64_t) ((uint64_t) x + (uint64_t) y);
-					ovf = ((x ^ r) & (y ^ r)) < 0;
-				}
-				else if (code == CBP_SUB)
-				{
-					r = (int64_t) ((uint64_t) x - (uint64_t) y);
-					ovf = ((x ^ y) & (x ^ r)) < 0;
-				}
-				else
-				{
-					r = (int64_t) ((uint64_t) x * (uint64_t) y);
-					ovf = __mul64hi(x, y) != (r >> 63);
-				}
 				if (alive && !n && ovf)
 					atomicExch(status, CBGPU_ERR_OVERFLOW);
 				sp--;
@@ -322,6 +312,50 @@ sink_store(void *col, int type, uint64_t pos, int64_t v)
 			break;
 		default:
 			((uint8_t *) col)[pos] = (uint8_t) v;
+	}
+}
+
+/* One lane reserves n rows for destination d and gets the position of the first.  out_count[d] counts every row routed to d,
+ * stored or not: a staged Motion's retry sizes its exact buffers from these counts.  A direct Motion takes its slice of the
+ * destination's window from that segment's own counter; the local count stays as a statistic.  Rows from seg_cap[d] on are
+ * not stored (sink_put_row): a full Motion destination is not an error, the host redoes the pass with exact sizes. */
+__device__ __forceinline__ unsigned long long
+sink_reserve(const SinkOut &o, int d, unsigned n, int *status)
+{
+	unsigned long long pos = atomicAdd(o.out_count + d, (unsigned long long) n);
+
+	if (o.part_cols)
+		pos = atomicAdd_system(o.part_counts[d], (unsigned long long) n);
+	if ((int64_t) (pos + n) > o.seg_cap[d])
+	{
+		if (o.part_flags)
+			atomicOr(o.part_flags, CBGPU_DX_OVERFLOW);
+		else
+			atomicExch(status, CBGPU_ERR_NOMEM);
+	}
+	return pos;
+}
+
+/* Store the row reserved at `pos` for destination d: column c's value is val(c), and bit c of nullbits its NULL flag, which
+ * goes to the column's NULL bytes; a NULL for a column that has none is refused. */
+template <class Val>
+__device__ __forceinline__ void
+sink_put_row(const SinkOut &o, int d, unsigned long long pos, Val val, uint64_t nullbits, int *status)
+{
+	const bool	direct = o.part_cols != NULL;
+	const uint64_t dst = direct ? pos : (uint64_t) o.seg_base[d] + pos;
+
+	if ((int64_t) pos >= o.seg_cap[d])
+		return;
+	for (int c = 0; c < o.nout; c++)
+	{
+		uint8_t    *nulls = !direct ? o.outnull[c] : ((o.part_nullmask >> c) & 1) ? o.part_nulls[d * o.nout + c] : NULL;
+
+		sink_store(direct ? o.part_cols[d * o.nout + c] : o.outcol[c], o.outtype[c], dst, val(c));
+		if (nulls)
+			nulls[dst] = (nullbits >> c) & 1;
+		else if ((nullbits >> c) & 1)
+			atomicExch(status, CBGPU_ERR_INVALID);
 	}
 }
 

@@ -113,33 +113,20 @@ struct PcParams
 	int32_t		fuse0;
 	uint32_t	smem_table_bytes;	/* shared-memory tables of the mode 2 probes, all together             */
 	/* sink */
-	int32_t		sink_kind;		/* CBP_SINK_AGG or CBP_SINK_MATERIALIZE                               */
+	int32_t		sink_kind;		/* CBP_SINK_AGG, CBP_SINK_MATERIALIZE or CBP_SINK_PARTITION          */
 	AggDev		agg;
 	int32_t		nkeys;
 	PcCol		key[CBP_MAX_KEYS];
+	int32_t		keytype[CBP_MAX_KEYS];
+	const uint32_t *keydict[CBP_MAX_KEYS];
 	int32_t		naccs;
 	int32_t		acc_term[CBP_MAX_AGGS];	/* -1 = count, else index of the value term               */
 	int32_t		nterms;
 	int32_t		term_kind[2];	/* 0 = column a, 1 = a * (k - b), 2 = a - b, 3 = a + b                */
 	PcCol		term_a[2], term_b[2];
 	long long	term_k[2];
-	int32_t		nout;
-	PcCol		out[PC_MAXOUT];
-	void	   *outcol[PC_MAXOUT];
-	int32_t		outtype[PC_MAXOUT];
-	unsigned long long *out_count;
-	int64_t		out_capacity;
-	/* PARTITION: cdbhash over the first nhash output columns picks the destination segment */
-	int32_t		nhash;
-	int32_t		hashtype[CBP_MAX_KEYS];
-	const uint32_t *hashdict[CBP_MAX_KEYS];
-	int32_t		nsegs;
-	int64_t		seg_capacity;
-	void *const *part_cols;		/* direct Motion: destination d's column c at part_cols[d * nout + c]  */
-	unsigned long long *const *part_counts;
-	int32_t    *part_flags;		/* a full destination ORs CBGPU_DX_OVERFLOW in here (NULL: status word) */
-	int64_t		seg_base[64];
-	int64_t		seg_cap[64];
+	PcCol		out[PC_MAXOUT];	/* MATERIALIZE / PARTITION: output column c's values ...              */
+	SinkOut		sink;			/* ... and where the rows go                                          */
 	int		   *status;
 };
 
@@ -370,6 +357,9 @@ pc_stage_table(const PcProbe &pr, int j, PcQ Q, unsigned base, unsigned n, uint3
 __device__ __noinline__ void
 pc_stage_sink(const PcParams &P, PcQ Q, unsigned base, unsigned n, unsigned long long *s_obase, PcPart *part)
 {
+	const SinkOut &O = P.sink;
+	int64_t		kv[CBP_MAX_KEYS];	/* the group or the hash keys of one row */
+
 	if (P.sink_kind == CBP_SINK_AGG)
 	{
 		for (unsigned b = 0; b < n; b += PC_THREADS)
@@ -379,46 +369,28 @@ pc_stage_sink(const PcParams &P, PcQ Q, unsigned base, unsigned n, unsigned long
 			if (i < n)
 			{
 				const uint32_t e = base + i;
-				int64_t		kv[CBP_MAX_KEYS];
-				uint32_t	h = 0;
 
-				/* TupleHashTableHash_internal (executor/execGrouping.c:437-495) */
 				for (int k = 0; k < P.nkeys; k++)
-				{
 					kv[k] = pc_load(P.key[k], Q, e);
-					h = pg_hash_combine(h, pg_hash_datum(P.key[k].type, kv[k], P.key[k].dict), false);
-				}
-				h = pg_murmurhash32(h);
+				const uint32_t h = agg_group_hash(P.nkeys, P.keytype, P.keydict, kv, 0);
 				int64_t		tv[2] = {0, 0};
 
 				for (int t = 0; t < P.nterms; t++)
 				{
-					int64_t		a = pc_load(P.term_a[t], Q, e);
+					const int64_t a = pc_load(P.term_a[t], Q, e);
+					bool		ovf = false,
+								ovf_mul = false;
 
 					if (P.term_kind[t] == 1)
-					{
-						int64_t		bb = pc_load(P.term_b[t], Q, e);
-						int64_t		k = P.term_k[t];
-						int64_t		d = (int64_t) ((uint64_t) k - (uint64_t) bb);
-						int64_t		r = (int64_t) ((uint64_t) a * (uint64_t) d);
-
-						/* numeric_mul / numeric_sub are exact; a product that leaves 64 bits is refused */
-						if ((((k ^ bb) & (k ^ d)) < 0) || (__mul64hi(a, d) != (r >> 63)))
-							atomicExch(P.status, CBGPU_ERR_OVERFLOW);
-						tv[t] = r;
-					}
-					else if (P.term_kind[t] >= 2)
-					{
-						const int64_t bb = pc_load(P.term_b[t], Q, e);
-						const int64_t r = P.term_kind[t] == 2 ? (int64_t) ((uint64_t) a - (uint64_t) bb) : (int64_t) ((uint64_t) a + (uint64_t) bb);
-
-						/* int8mi / int8pl raise "bigint out of range" (utils/adt/int8.c:448,427): refused */
-						if (P.term_kind[t] == 2 ? (((a ^ bb) & (a ^ r)) < 0) : ((~(a ^ bb) & (a ^ r)) < 0))
-							atomicExch(P.status, CBGPU_ERR_OVERFLOW);
-						tv[t] = r;
-					}
+						tv[t] = i64_mul_ovf(a, i64_sub_ovf(P.term_k[t], pc_load(P.term_b[t], Q, e), &ovf), &ovf_mul);
+					else if (P.term_kind[t] == 2)
+						tv[t] = i64_sub_ovf(a, pc_load(P.term_b[t], Q, e), &ovf);
+					else if (P.term_kind[t] == 3)
+						tv[t] = i64_add_ovf(a, pc_load(P.term_b[t], Q, e), &ovf);
 					else
 						tv[t] = a;
+					if (ovf || ovf_mul)
+						atomicExch(P.status, CBGPU_ERR_OVERFLOW);
 				}
 				int			slot = agg_find_or_insert(P.agg, h, kv, 0);
 
@@ -443,65 +415,32 @@ pc_stage_sink(const PcParams &P, PcQ Q, unsigned base, unsigned n, unsigned long
 		__syncthreads();
 		for (unsigned i = threadIdx.x; i < n; i += PC_THREADS)
 		{
-			uint32_t	h = 0;
-
-			for (int k = 0; k < P.nhash; k++)
-				h = pg_hash_combine(h, pg_hash_datum(P.hashtype[k], pc_load(P.out[k], Q, base + i), P.hashdict[k]), false);
-			const int	seg = pg_jump_consistent_hash(h, P.nsegs);
+			for (int k = 0; k < O.nhash; k++)
+				kv[k] = pc_load(P.out[k], Q, base + i);
+			const int	seg = cdb_route(O.nhash, O.hashtype, O.hashdict, kv, 0, O.nsegs);
 
 			part->seg[i] = (uint8_t) seg;
 			part->rank[i] = (uint16_t) atomicAdd(&part->count[seg], 1u);
 		}
 		__syncthreads();
-		if (threadIdx.x < P.nsegs && part->count[threadIdx.x])
-		{
-			unsigned long long b = atomicAdd(P.out_count + threadIdx.x, (unsigned long long) part->count[threadIdx.x]);
-
-			/* direct Motion: the slice is reserved in the DESTINATION segment's buffer, over NVLink */
-			if (P.part_cols)
-				b = atomicAdd_system(P.part_counts[threadIdx.x], (unsigned long long) part->count[threadIdx.x]);
-			part->base[threadIdx.x] = b;
-			if ((int64_t) (b + part->count[threadIdx.x]) > P.seg_cap[threadIdx.x])
-			{
-				/* a full Motion destination is not an error: the host redoes the pass with exact sizes */
-				if (P.part_flags)
-					atomicOr(P.part_flags, CBGPU_DX_OVERFLOW);
-				else
-					atomicExch(P.status, CBGPU_ERR_NOMEM);
-			}
-		}
+		if (threadIdx.x < O.nsegs && part->count[threadIdx.x])
+			part->base[threadIdx.x] = sink_reserve(O, threadIdx.x, part->count[threadIdx.x], P.status);
 		__syncthreads();
 		for (unsigned i = threadIdx.x; i < n; i += PC_THREADS)
 		{
 			const int	seg = part->seg[i];
-			const unsigned long long pos = part->base[seg] + part->rank[i];
 
-			if ((int64_t) pos < P.seg_cap[seg])
-			{
-				const uint64_t dst = P.part_cols ? pos : (uint64_t) P.seg_base[seg] + pos;
-
-				for (int c = 0; c < P.nout; c++)
-					sink_store(P.part_cols ? P.part_cols[seg * P.nout + c] : P.outcol[c], P.outtype[c], dst, pc_load(P.out[c], Q, base + i));
-			}
+			sink_put_row(O, seg, part->base[seg] + part->rank[i], [&](int c) { return pc_load(P.out[c], Q, base + i); }, 0, P.status);
 		}
 	}
 	else
 	{
 		/* one reservation of n output rows per run, then coalesced stores */
 		if (threadIdx.x == 0)
-			*s_obase = atomicAdd(P.out_count, (unsigned long long) n);
+			*s_obase = sink_reserve(O, 0, n, P.status);
 		__syncthreads();
-		const unsigned long long ob = *s_obase;
-
-		if ((int64_t) (ob + n) > P.out_capacity)
-		{
-			if (threadIdx.x == 0)
-				atomicExch(P.status, CBGPU_ERR_NOMEM);
-		}
-		else
-			for (unsigned i = threadIdx.x; i < n; i += PC_THREADS)
-				for (int c = 0; c < P.nout; c++)
-					sink_store(P.outcol[c], P.outtype[c], ob + i, pc_load(P.out[c], Q, base + i));
+		for (unsigned i = threadIdx.x; i < n; i += PC_THREADS)
+			sink_put_row(O, 0, *s_obase + i, [&](int c) { return pc_load(P.out[c], Q, base + i); }, 0, P.status);
 	}
 }
 
@@ -1274,7 +1213,8 @@ cb_try_probe_chain(cbgpu_ctx *ctx, const CbPipeline *p, const PipeDev *d, const 
 			if (!xm_is_load(&x, x.stack[k], &col) || !pc_col(p, col, &P.key[k], base))
 				PC_REJECT(17);
 			P.key[k].type = s->keytype[k];
-			P.key[k].dict = s->key_dict_hash[k];
+			P.keytype[k] = d->sink.keytype[k];
+			P.keydict[k] = d->sink.keydict[k];
 		}
 		P.naccs = s->naccs;
 		for (int a = 0; a < s->naccs; a++)
@@ -1333,37 +1273,14 @@ cb_try_probe_chain(cbgpu_ctx *ctx, const CbPipeline *p, const PipeDev *d, const 
 	{
 		if (s->nout > PC_MAXOUT || x.depth != s->nout)
 			PC_REJECT(23);
-		P.nout = s->nout;
 		for (int c = 0; c < s->nout; c++)
 		{
 			int			col;
 
-			if (!xm_is_load(&x, x.stack[c], &col) || !pc_col(p, col, &P.out[c], base) || d->sink.outnull[c])
+			if (!xm_is_load(&x, x.stack[c], &col) || !pc_col(p, col, &P.out[c], base) || d->sink.out.outnull[c])
 				PC_REJECT(24);
-			P.outcol[c] = d->sink.outcol[c];
-			P.outtype[c] = d->sink.outtype[c];
 		}
-		P.out_count = d->sink.out_count;
-		P.out_capacity = d->sink.out_capacity;
-		if (s->kind == CBP_SINK_PARTITION)
-		{
-			P.nhash = d->sink.nhash;
-			P.nsegs = d->sink.nsegs;
-			P.seg_capacity = d->sink.seg_capacity;
-			P.part_cols = d->sink.part_cols;
-			P.part_counts = d->sink.part_counts;
-			P.part_flags = d->sink.part_flags;
-			for (int g = 0; g < P.nsegs && g < 64; g++)
-			{
-				P.seg_base[g] = d->sink.seg_base[g];
-				P.seg_cap[g] = d->sink.seg_cap[g];
-			}
-			for (int k = 0; k < P.nhash; k++)
-			{
-				P.hashtype[k] = d->sink.hashtype[k];
-				P.hashdict[k] = d->sink.hashdict[k];
-			}
-		}
+		P.sink = d->sink.out;
 	}
 
 	/* scan-level runtime filters.  The reference pushes a Bloom filter per integer hash-clause column down to the

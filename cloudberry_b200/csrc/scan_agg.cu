@@ -461,12 +461,7 @@ k_small_commit(const __grid_constant__ SmallAggParams P, int G, int nblocks)
 		if (key == 0 || cnt == 0)
 			continue;
 		int64_t		kv[2] = {(int64_t) (key & 0xff), (int64_t) ((key >> 8) & 0xff)};
-		uint32_t	h = 0;
-
-		for (int k = 0; k < P.nkeys; k++)
-			h = pg_hash_combine(h, pg_hash_datum(P.keytype[k], kv[k], P.keydict[k]), false);
-		h = pg_murmurhash32(h);
-		int			slot = agg_find_or_insert(P.agg, h, kv, 0);
+		int			slot = agg_find_or_insert(P.agg, agg_group_hash(P.nkeys, P.keytype, P.keydict, kv, 0), kv, 0);
 
 		if (slot < 0)
 			continue;

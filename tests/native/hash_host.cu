@@ -22,4 +22,12 @@ uint64_t	hh_slot_entry(uint32_t tag, uint32_t row) { return ht_slot_entry(tag, r
 int			hh_slot_empty(uint64_t e) { return ht_slot_empty(e); }
 uint32_t	hh_slot_row(uint64_t e) { return ht_slot_row(e); }
 int			hh_tag_match(uint64_t e, uint32_t tag) { return ht_tag_match(e, tag); }
+int64_t		hh_group_key(int type, int64_t v) { return agg_group_key(type, v); }
+uint32_t	hh_group_hash(int n, const int32_t *types, const uint32_t *const *dicts, const int64_t *keys, uint32_t knull)
+{ return agg_group_hash(n, types, dicts, keys, knull); }
+int32_t		hh_cdb_route(int n, const int32_t *types, const uint32_t *const *dicts, const int64_t *keys, uint32_t knull, int32_t nsegs)
+{ return cdb_route(n, types, dicts, keys, knull, nsegs); }
+int64_t		hh_add_ovf(int64_t x, int64_t y, int *ovf) { bool o; int64_t r = i64_add_ovf(x, y, &o); *ovf = o; return r; }
+int64_t		hh_sub_ovf(int64_t x, int64_t y, int *ovf) { bool o; int64_t r = i64_sub_ovf(x, y, &o); *ovf = o; return r; }
+int64_t		hh_mul_ovf(int64_t x, int64_t y, int *ovf) { bool o; int64_t r = i64_mul_ovf(x, y, &o); *ovf = o; return r; }
 }

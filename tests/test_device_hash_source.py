@@ -1,6 +1,7 @@
 """The hash functions the kernels inline, as SOURCE (cloudberry_b200/csrc/common.cuh, __host__ __device__), compiled for the host
-and held against the reference's own code (not gpu): hashint4 / hashint8 / hashfloat8 / hashbpchar, murmurhash32, the
-rotate-xor key combination of nodeHash.c / execGrouping.c / cdbhash.c, and jump_consistent_hash through cdbhashreduce.
+and held against the reference's own code (not gpu): hashint4 / hashint8 / hashfloat8 / hashbpchar, murmurhash32 and
+jump_consistent_hash, and the compositions every sink calls - the Motion route (cdb_route: cdbhash, cdbhashreduce) and the
+group hash (agg_group_hash: TupleHashTableHash_internal) - plus the checked int64 add / sub / mul of the kernels' arithmetic.
 On the device the same text runs with __ddiv_rn / __dmul_rn in the jump hash (IEEE, no contraction), which
 tests/test_gpu_multirank.py and the Motion tests check against the oracle's routes.  The join table's slot format (ht_slot_entry,
 ht_probe_tag, ht_tag_match, ht_key_in_domain) is the same kind of source and is held against its rule over the key sets
@@ -35,7 +36,12 @@ def host(tmp_path_factory):
         getattr(H, name).argtypes = args
     H.hh_jump_consistent_hash.restype = C.c_int32
     H.hh_jump_consistent_hash.argtypes = [C.c_uint64, C.c_int32]
+    keys = [C.c_int, C.POINTER(C.c_int32), C.POINTER(C.c_void_p), C.POINTER(C.c_int64), C.c_uint32]
+    ovf = [C.c_int64, C.c_int64, C.POINTER(C.c_int)]
     for name, res, args in (("hh_jh_int8", C.c_uint32, [C.c_int64]), ("hh_jh_mix32", C.c_uint32, [C.c_uint32]),
+                            ("hh_group_key", C.c_int64, [C.c_int, C.c_int64]), ("hh_group_hash", C.c_uint32, keys),
+                            ("hh_cdb_route", C.c_int32, keys + [C.c_int32]), ("hh_add_ovf", C.c_int64, ovf),
+                            ("hh_sub_ovf", C.c_int64, ovf), ("hh_mul_ovf", C.c_int64, ovf),
                             ("hh_key_in_domain", C.c_int, [C.c_int32, C.c_int64]),
                             ("hh_probe_tag", C.c_uint32, [C.c_int32, C.c_uint32, C.c_int64]),
                             ("hh_slot_entry", C.c_uint64, [C.c_uint32, C.c_uint32]), ("hh_slot_empty", C.c_int, [C.c_uint64]),
@@ -76,6 +82,8 @@ def test_stored_reference_answers(host):
     for known, nseg in ((KNOWN_SEG8, 8), (KNOWN_SEG3, 3)):
         for k, seg in known.items():
             assert H.hh_jump_consistent_hash(H.hh_hash_combine(0, H.hh_hash_uint32(k), 0), nseg) == seg
+            for t in (CB_INT4, CB_DATE):
+                assert _call_keys(H.hh_cdb_route, [t], [k - (1 << 32) if k >= (1 << 31) else k], [0], None, nseg) == seg
 
 
 def _bits(f):
@@ -84,6 +92,45 @@ def _bits(f):
 
 def _s64(u):
     return u - (1 << 64) if u >= (1 << 63) else u
+
+
+# CbTypeId (include/cb_plan.h) of the kernels' key types
+CB_INT4, CB_INT8, CB_DATE, CB_BPCHAR1, CB_DICT32, CB_FLOAT8 = 1, 2, 3, 5, 7, 8
+REF_KIND = {CB_INT4: INT4, CB_DATE: INT4, CB_INT8: INT8, CB_FLOAT8: FLOAT8, CB_BPCHAR1: BPCHAR, CB_DICT32: BPCHAR}
+WORDS = ["", "A", "ASIA", "MACHINERY", "1-URGENT", "a longer string than twelve bytes", "Brand#13 ", "\u00e9t\u00e9"]
+
+
+def _call_keys(fn, types, vals, nulls, dicts, *extra):
+    """fn(nkeys, types, dicts, keys, knull, *extra) over ctypes arrays; dicts[k] is a list of per-code hashes or None"""
+    n = len(types)
+    tables = [(C.c_uint32 * len(d))(*d) if d else None for d in (dicts or [None] * n)]
+    ptrs = (C.c_void_p * n)(*[C.cast(t, C.c_void_p) if t is not None else None for t in tables])
+    knull = sum(1 << k for k, nul in enumerate(nulls) if nul)
+    return fn(n, (C.c_int32 * n)(*types), ptrs, (C.c_int64 * n)(*vals), knull, *extra)
+
+
+def _random_keys(rng, R):
+    """1-4 keys of the kernels' key types with NULLs; per key: type, device value, the reference's (bits, string), dictionary"""
+    word_hash = [R.ref_hash_datum(BPCHAR, 0, w.encode(), len(w.encode())) for w in WORDS]
+    keys = []
+    for _ in range(rng.randrange(1, 5)):
+        t = rng.choice([CB_INT4, CB_DATE, CB_INT8, CB_FLOAT8, CB_BPCHAR1, CB_DICT32])
+        d, s = None, None
+        if t in (CB_INT4, CB_DATE):
+            v = rng.choice([0, -1, -2 ** 31, 2 ** 31 - 1, rng.getrandbits(32) - 2 ** 31])
+        elif t == CB_INT8:
+            v = rng.choice([0, -1, -2 ** 63, 2 ** 63 - 1, rng.getrandbits(64) - 2 ** 63])
+        elif t == CB_FLOAT8:
+            v = _s64(rng.choice([_bits(0.0), _bits(-0.0), 0x7ff8000000000000, 0xfff0000000000001, 0x7ff0000000000123,
+                                 _bits(float("inf")), _bits(rng.uniform(-1e9, 1e9))]))
+        elif t == CB_BPCHAR1:
+            v = rng.randrange(1, 256)
+            s = bytes([v])
+        else:
+            v = rng.randrange(len(WORDS))
+            d, s = word_hash, WORDS[v].encode()
+        keys.append((t, v, s, d, 1 if rng.random() < 0.15 else 0))
+    return keys
 
 
 def test_type_hash_functions(libs):
@@ -112,32 +159,68 @@ def test_murmur_and_key_combination(libs):
     for _ in range(5000):
         x = rng.getrandbits(32)
         assert H.hh_murmurhash32(x) == P.ref_murmurhash32(x)
-    # the Motion's use of the combination: cdbhash over several keys, NULLs included, then the jump hash
-    kinds = [INT4, INT8, FLOAT8]
-    for _ in range(4000):
-        nk = rng.randrange(1, 5)
-        nseg = rng.choice([1, 2, 3, 4, 8, 16, 48, 64, 1000])
-        ks = [rng.choice(kinds) for _ in range(nk)]
-        nulls = [1 if rng.random() < 0.15 else 0 for _ in range(nk)]
-        vals = []
-        acc = 0
-        for k, nul in zip(ks, nulls):
-            if k == INT4:
-                v = rng.getrandbits(32) - 2 ** 31
-                h = H.hh_hash_uint32(v & 0xffffffff)
-            elif k == INT8:
-                v = rng.getrandbits(64) - 2 ** 63
-                h = H.hh_hashint8(v)
-            else:
-                b = _bits(rng.uniform(-1e9, 1e9))
-                v = _s64(b)
-                h = H.hh_hashfloat8(b)
-            vals.append(v)
-            acc = H.hh_hash_combine(acc, h, nul)
-        want = R.ref_cdbhash_segment(nk, (C.c_int * nk)(*ks), (C.c_int64 * nk)(*vals), None, (C.c_uint8 * nk)(*nulls), nseg)
+        nseg = rng.choice([1, 2, 3, 8, 48, 64, 1000])
+        assert H.hh_jump_consistent_hash(x, nseg) == R.ref_jump_consistent_hash(x, nseg)
+    # the Motion's route as the kernels compile it (cdb_route: cdbhash over the keys, then cdbhashreduce) against the
+    # reference's own evalHashKey on the same keys: int4, date, int8, float8 (signed zeros and NaN payloads), bpchar(1),
+    # dictionary codes whose per-code table holds hashbpchar of each string, NULLs, 1-64 segments and a few more
+    for i in range(6000):
+        nseg = 1 + i % 64 if i < 5000 else rng.choice([65, 100, 1000, 4096])
+        keys = _random_keys(rng, R)
+        ts, vs, ss, ds, ns = zip(*keys)
+        nk = len(keys)
+        strs = (C.c_char_p * nk)(*ss)
+        want = R.ref_cdbhash_segment(nk, (C.c_int * nk)(*[REF_KIND[t] for t in ts]), (C.c_int64 * nk)(*vs), strs,
+                                     (C.c_uint8 * nk)(*ns), nseg)
         assert want >= 0
-        assert H.hh_jump_consistent_hash(acc, nseg) == want, (ks, vals, nulls, nseg)
-        assert R.ref_jump_consistent_hash(acc, nseg) == want
+        assert _call_keys(H.hh_cdb_route, ts, vs, ns, ds, nseg) == want, (keys, nseg)
+
+
+def test_group_hash(libs, host):
+    """agg_group_hash against TupleHashTableHash_internal composed of the reference's pieces: its hash functions, the
+    rotate-xor with NULLs contributing nothing, then libpg_hashfn's murmurhash32"""
+    H, R, P = libs
+    rng = random.Random(80)
+    for _ in range(4000):
+        keys = _random_keys(rng, R)
+        want = 0
+        for t, v, s, d, nul in keys:
+            want = ((want << 1) | (want >> 31)) & 0xffffffff
+            if not nul:
+                want ^= R.ref_hash_datum(REF_KIND[t], v, s, len(s) if s else 0)
+        ts, vs, _, ds, ns = zip(*keys)
+        assert _call_keys(H.hh_group_hash, ts, vs, ns, ds) == P.ref_murmurhash32(want), keys
+
+
+def test_group_key_float8(host):
+    """float8eq's groups: -0.0 and +0.0 are one key, every NaN payload is one key, and they hash alike (with a second key)"""
+    H = host
+    for same in ([_bits(0.0), _bits(-0.0)], [0x7ff8000000000000, 0xfff8000000000000, 0x7ff0000000000001, 0xffffffffffffffff]):
+        ks = {H.hh_group_key(CB_FLOAT8, _s64(b)) for b in same}
+        assert len(ks) == 1
+        hs = {_call_keys(H.hh_group_hash, [CB_FLOAT8, CB_INT4], [_s64(b), 7], [0, 0], None) for b in same}
+        assert len(hs) == 1
+    for b in (_bits(1.5), _bits(float("inf")), _bits(float("-inf")), 1):
+        assert H.hh_group_key(CB_FLOAT8, _s64(b)) == _s64(b)
+    assert H.hh_group_key(CB_INT8, _s64(_bits(-0.0))) == _s64(_bits(-0.0))
+
+
+def test_checked_int64_arithmetic(host):
+    """i64_add_ovf / i64_sub_ovf / i64_mul_ovf: the wrapped result and whether the exact one leaves int64 (int8pl / int8mi /
+    int8mul's "bigint out of range")"""
+    H = host
+    rng = random.Random(81)
+    edges = [0, 1, 2 ** 31, 2 ** 32, 2 ** 62]
+    vals = sorted({s * e for e in edges for s in (1, -1)} | {-2 ** 63, 2 ** 63 - 1, 2 ** 63 - 2, -2 ** 63 + 1, 3037000499,
+                                                             3037000500})
+    vals += [rng.getrandbits(64) - 2 ** 63 for _ in range(60)] + [rng.getrandbits(33) - 2 ** 32 for _ in range(30)]
+    for x in vals:
+        for y in vals:
+            for fn, exact in ((H.hh_add_ovf, x + y), (H.hh_sub_ovf, x - y), (H.hh_mul_ovf, x * y)):
+                o = C.c_int(-1)
+                r = fn(x, y, C.byref(o))
+                assert r == _s64(exact & (2 ** 64 - 1)), (fn.__name__, x, y)
+                assert o.value == (not -2 ** 63 <= exact < 2 ** 63), (fn.__name__, x, y)
 
 
 def test_join_slot_format(host):

@@ -58,21 +58,24 @@ def test_q5_reference_expected(ctx, golden_dev, generic):
     ex.close()
 
 
-@pytest.mark.parametrize("nsegs", [2, 3])
-def test_q1_two_stage_on_segments(ctx, oracle, golden, nsegs):
-    """partial agg -> Redistribute Motion (cdbhash + jump hash on device) -> final agg -> gather."""
+@pytest.mark.parametrize("nsegs,generic", [pytest.param(n, g, id="%d%s" % (n, "-generic" if g else ""))
+                                           for g in (False, True) for n in (2, 3)])
+def test_q1_two_stage_on_segments(ctx, oracle, golden, nsegs, generic):
+    """partial agg -> Redistribute Motion (cdbhash + jump hash on device) -> final agg -> gather, through the fused
+    kernels' sinks and through the generic kernel's."""
     rels, exp = golden
     segs = shard(oracle, rels, nsegs)
     dsegs = [to_device(ctx, s) for s in segs]
-    cl = capi.Cluster(ctx, dsegs)
+    cl = capi.Cluster(ctx, dsegs, force_generic=generic)
     res = cl.run(tpch.q1_plan(nsegs))
     assert tpch.format_q1(res.rows) == exp["q1"]
     assert set(res.segments) == {0}
     cl.close()
 
 
-@pytest.mark.parametrize("replicated", [True, False])
-def test_q3_q5_on_segments(ctx, oracle, golden, replicated):
+@pytest.mark.parametrize("replicated,generic", [pytest.param(r, g, id="%s%s" % (r, "-generic" if g else ""))
+                                               for g in (False, True) for r in (True, False)])
+def test_q3_q5_on_segments(ctx, oracle, golden, replicated, generic):
     rels, exp = golden
     nsegs = 3
     dist = dict(tpch.DIST_KEY)
@@ -81,7 +84,7 @@ def test_q3_q5_on_segments(ctx, oracle, golden, replicated):
         dist["supplier"] = "s_suppkey"
     segs = shard(oracle, rels, nsegs, dist)
     dsegs = [to_device(ctx, s) for s in segs]
-    cl = capi.Cluster(ctx, dsegs)
+    cl = capi.Cluster(ctx, dsegs, force_generic=generic)
     seg = exp["dict"]["c_mktsegment_dict"].index("MACHINERY")
     res = cl.run(tpch.q3_plan(seg, nsegs, customer_replicated=replicated))
     assert tpch.format_q3(res.rows) == exp["q3"]
