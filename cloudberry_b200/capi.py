@@ -501,6 +501,8 @@ def ex():
         L.cb_cluster_next.argtypes = [vp]
         L.cb_cluster_current_segment.restype = C.c_int32
         L.cb_cluster_current_segment.argtypes = [vp]
+        L.cb_cluster_root.restype = C.POINTER(CbPlanState)
+        L.cb_cluster_root.argtypes = [vp, C.c_int32]
         L.cb_cluster_end.argtypes = [vp]
         L.cb_cluster_destroy.argtypes = [vp]
         L.cb_cluster_error.restype = C.c_char_p
@@ -829,6 +831,7 @@ class Result:
         self.states = []
         self.segments = []
         self.instrument = {}
+        self.segment_instrument = []      # Cluster.run: one instrument dict per segment
 
 
 def _collect_instrument(ps, out):
@@ -954,6 +957,9 @@ class Cluster:
                 res.rows.append(row)
                 res.states.append(st)
                 res.segments.append(int(E.cb_cluster_current_segment(self.h)))
+            for s in range(self.nsegs):
+                res.segment_instrument.append({})
+                _collect_instrument(E.cb_cluster_root(self.h, s), res.segment_instrument[s])
         finally:
             E.cb_cluster_end(self.h)
         return res

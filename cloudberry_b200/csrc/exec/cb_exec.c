@@ -2763,7 +2763,14 @@ motion_send_side(CbPlanState *ps, cbgpu_rel **send, int64_t *counts, int64_t *of
 		offsets[0] = 0;
 		return CBGPU_OK;
 	}
-	/* hash motion: PARTITION sink = evalHashKey (nodeMotion.c:1088) + per-destination buffers */
+	/* hash motion: PARTITION sink = evalHashKey (nodeMotion.c:1088) + per-destination buffers.  Those buffers, the
+	 * sink's and the staged pass's per-destination bases and capacities, hold at most 64 destinations.  Every segment
+	 * refuses here alike, before any exchange is entered: there is none to abandon. */
+	if (nsegs > 64)
+	{
+		p->xstage = 2;
+		return es_fail(es, CBGPU_ERR_UNSUPPORTED, "hash Motion over more than 64 segments (%d)", nsegs);
+	}
 	pl = &s->pipe;
 	saved_nops = pl->nops;
 	if (m->nhashExprs < 1 || m->nhashExprs > CBP_MAX_KEYS)
@@ -2881,8 +2888,6 @@ open_motion(CbPlanState *ps, CbStream **out)
 		CbInterconnect *ic = es->es_interconnect;
 		int			rc;
 
-		if (es->es_numsegments > 64)
-			return es_fail(es, CBGPU_ERR_UNSUPPORTED, "more than 64 segments");
 		memset(counts, 0, sizeof(counts));
 		memset(offsets, 0, sizeof(offsets));
 		rc = motion_send_side(ps, &send, counts, offsets);
@@ -3999,6 +4004,12 @@ int32_t
 cb_cluster_current_segment(CbCluster *c)
 {
 	return c->cur;
+}
+
+CbPlanState *
+cb_cluster_root(CbCluster *c, int32_t seg)
+{
+	return (seg >= 0 && seg < c->nsegs) ? c->roots[seg] : NULL;
 }
 
 const char *

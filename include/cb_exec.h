@@ -222,6 +222,8 @@ int			cb_cluster_init_plan(CbCluster *c, CbPlan *plan);
  * receives from a Gather Motion runs on segment 0 only) */
 CbTupleTableSlot *cb_cluster_next(CbCluster *c);
 int32_t		cb_cluster_current_segment(CbCluster *c);
+/* root PlanState of one segment's copy of the plan, from cb_cluster_init_plan to cb_cluster_end (its instrumentation) */
+CbPlanState *cb_cluster_root(CbCluster *c, int32_t seg);
 void		cb_cluster_end(CbCluster *c);
 void		cb_cluster_destroy(CbCluster *c);
 const char *cb_cluster_error(CbCluster *c);

@@ -3,7 +3,7 @@ and held against the reference's own code (not gpu): hashint4 / hashint8 / hashf
 jump_consistent_hash, and the compositions every sink calls - the Motion route (cdb_route: cdbhash, cdbhashreduce) and the
 group hash (agg_group_hash: TupleHashTableHash_internal) - plus the checked int64 add / sub / mul of the kernels' arithmetic.
 On the device the same text runs with __ddiv_rn / __dmul_rn in the jump hash (IEEE, no contraction), which
-tests/test_gpu_multirank.py and the Motion tests check against the oracle's routes.  The join table's slot format (ht_slot_entry,
+tests/test_gpu_motion_routes.py checks against the oracle's routes row by row, on every sink kernel and both transports.  The join table's slot format (ht_slot_entry,
 ht_probe_tag, ht_tag_match, ht_key_in_domain) is the same kind of source and is held against its rule over the key sets
 tests/test_gpu_join_routes.py joins on."""
 import ctypes as C
