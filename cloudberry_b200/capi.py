@@ -49,6 +49,26 @@ class CbgpuJoinFilter(C.Structure):
     _fields_ = [("ncols", C.c_int32), ("cols", C.POINTER(CbpColumn)), ("nops", C.c_int32), ("ops", C.POINTER(CbpOp))]
 
 
+# CbgpuSortNulls: where a sort key's NULLs come from
+SORT_NULLS_NONE, SORT_NULLS_MAP, SORT_NULLS_COUNT = range(3)
+
+
+class CbgpuSortKey(C.Structure):
+    """cbgpu_sort_key: one key of cbgpu_topn_select"""
+    _fields_ = [("col", C.c_int32), ("descending", C.c_int32), ("unsigned_cmp", C.c_int32), ("float8", C.c_int32),
+                ("nulls", C.c_int32), ("null_col", C.c_int32)]
+
+
+def topn_select(ctx, rel, keys, limit):
+    """cbgpu_topn_select: the row indices of the first min(limit, rows) rows of DeviceRelation rel in order.  keys: dicts of
+    CbgpuSortKey fields (col required)."""
+    arr = (CbgpuSortKey * max(len(keys), 1))(*[CbgpuSortKey(**k) for k in keys])
+    idx = (C.c_uint32 * max(min(limit, rel.nrows), 1))()
+    nout = C.c_int64(0)
+    ctx.check(ctx.L.cbgpu_topn_select(ctx.h, rel.h, arr, len(keys), limit, idx, C.byref(nout)))
+    return list(idx[:nout.value])
+
+
 # CbpOpCode
 (CBP_END, CBP_LOAD, CBP_CONST, CBP_ADD, CBP_SUB, CBP_MUL, CBP_FADD, CBP_FSUB, CBP_FMUL, CBP_I2F, CBP_EQ, CBP_NE, CBP_LT, CBP_LE,
  CBP_GT, CBP_GE, CBP_FEQ, CBP_FNE, CBP_FLT, CBP_FLE, CBP_FGT, CBP_FGE, CBP_AND, CBP_OR, CBP_NOT, CBP_FILTER, CBP_PROBE, CBP_DUP,
@@ -407,6 +427,7 @@ def gpu():
                                                   C.POINTER(i32)]),
             "cbgpu_topn": (C.c_int, [vp, vp, C.POINTER(i32), C.POINTER(i32), C.POINTER(i32), i32, i64, C.POINTER(C.c_uint32),
                                      C.POINTER(i64)]),
+            "cbgpu_topn_select": (C.c_int, [vp, vp, C.POINTER(CbgpuSortKey), i32, i64, C.POINTER(C.c_uint32), C.POINTER(i64)]),
             "cbgpu_rel_take_rows": (C.c_int, [vp, vp, vp, i64]),
             "cbgpu_dev_alloc": (C.c_int, [vp, C.c_size_t, C.POINTER(vp)]),
             "cbgpu_dev_write": (C.c_int, [vp, vp, C.c_size_t, vp]),

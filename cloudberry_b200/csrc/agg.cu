@@ -1056,3 +1056,471 @@ cbgpu_topn(cbgpu_ctx *ctx, cbgpu_rel *rel, const int32_t *keycols, const int32_t
 	*nout = n;
 	return CBGPU_OK;
 }
+
+/* ---------------------------------------------------------------------------------------------
+ * top-N for any LIMIT (cbgpu_topn_select).  Every key maps to a 64-bit image whose unsigned order is the sort order
+ * (topn_ukey, plus float8's order), preceded by a one-bit NULL digit: NULLS LAST ascending, FIRST descending, as rows_cmp and
+ * the merge receive order them.  One pass reduces each key's smallest and largest image and whether a NULL occurs; the host
+ * reads that back once and keeps the 8-bit digits that can vary.  An MSD radix select over those digits then takes the first
+ * min(limit, rows) rows - each pass counts the digit over the rows still tied, one CTA picks the digit where the remaining
+ * rank falls, and the tied rows are compacted stably - with no host synchronisation between passes: a pass after the one that
+ * decided exits at once.  What is still tied when the digits run out gives its lowest rows.  A stable LSD radix sort over the
+ * same digits orders the chosen rows.  Both start from row order, so equal keys keep it: the lower row index wins, as in
+ * topn_before.  Count and scatter are a stable counting sort modelled on k_ht_partition_count / _write.
+ * --------------------------------------------------------------------------------------------- */
+#define TSEL_THREADS 256
+#define TSEL_MAXDIGITS (TOPN_MAXKEYS * 9)
+#define TSEL_NULLDIGIT 64			/* the shift that names a key's NULL digit */
+
+struct TselKey
+{
+	const void *data;
+	const uint8_t *nullmap;			/* NULL map (1 = NULL), or NULL                                       */
+	const long long *ncol;			/* int8 column whose 0 means NULL, or NULL                            */
+	int32_t		type;
+	int32_t		desc;
+	int32_t		uns;
+	int32_t		f8;
+};
+
+struct TselKeys
+{
+	TselKey		k[TOPN_MAXKEYS];
+	int32_t		nkeys;
+};
+
+/* the selection's progress, on the device: pass p reads ntied[p] rows and leaves ntied[p + 1] */
+struct TselState
+{
+	unsigned long long need;		/* rows the tied set still owes the answer                            */
+	unsigned long long nsel;		/* rows chosen so far                                                 */
+	unsigned long long m;			/* min(limit, rows)                                                   */
+	unsigned long long ntied[TSEL_MAXDIGITS + 1];
+	int32_t		decided;			/* the pass that completed the selection, -1 while none has           */
+	int32_t		bucket[TSEL_MAXDIGITS];	/* each pass's chosen digit                                    */
+	int32_t		take[TSEL_MAXDIGITS];	/* 1: every row with that digit is chosen                      */
+};
+
+__device__ __forceinline__ unsigned long long
+tsel_image(const TselKey &k, uint32_t row, bool *isnull)
+{
+	unsigned long long u = (unsigned long long) cb_load_widen(k.data, k.type, row);
+
+	*isnull = (k.nullmap && __ldg(k.nullmap + row)) || (k.ncol && __ldg(k.ncol + row) == 0);
+	if (k.f8)
+	{
+		/* float8_cmp_internal: -0 = +0, every NaN equal and above +Infinity; then sign-magnitude to unsigned order */
+		if ((u << 1) == 0)
+			u = 0;
+		else if ((u & 0x7FF0000000000000ull) == 0x7FF0000000000000ull && (u & 0x000FFFFFFFFFFFFFull))
+			u = 0x7FF8000000000000ull;
+		u = (u >> 63) ? ~u : (u | 0x8000000000000000ull);
+	}
+	else if (!k.uns)
+		u ^= 0x8000000000000000ull;
+	return k.desc ? ~u : u;
+}
+
+/* digit `shift` of a row's key: the NULL digit, or 8 bits of the image (0 for a NULL, which its NULL digit already placed) */
+__device__ __forceinline__ int
+tsel_digit(const TselKey &k, int shift, uint32_t row)
+{
+	bool		isnull;
+	const unsigned long long u = tsel_image(k, row, &isnull);
+
+	if (shift == TSEL_NULLDIGIT)
+		return isnull != (k.desc != 0);
+	return isnull ? 0 : (int) ((u >> shift) & 255u);
+}
+
+/* red[0..3] smallest image, red[4..7] largest (non-NULL rows), red[8..11] nonzero when the key has a NULL */
+__global__ void __launch_bounds__(TSEL_THREADS)
+k_tsel_image(TselKeys p, int64_t n, unsigned long long *red)
+{
+	unsigned long long mn[TOPN_MAXKEYS],
+				mx[TOPN_MAXKEYS];
+	unsigned	nulls = 0;
+
+#pragma unroll
+	for (int i = 0; i < TOPN_MAXKEYS; i++)
+	{
+		mn[i] = ~0ull;
+		mx[i] = 0;
+	}
+	for (int64_t r = (int64_t) blockIdx.x * blockDim.x + threadIdx.x; r < n; r += (int64_t) gridDim.x * blockDim.x)
+#pragma unroll
+		for (int i = 0; i < TOPN_MAXKEYS; i++)
+			if (i < p.nkeys)
+			{
+				bool		isnull;
+				const unsigned long long u = tsel_image(p.k[i], (uint32_t) r, &isnull);
+
+				if (isnull)
+					nulls |= 1u << i;
+				else
+				{
+					mn[i] = u < mn[i] ? u : mn[i];
+					mx[i] = u > mx[i] ? u : mx[i];
+				}
+			}
+	nulls = __reduce_or_sync(0xffffffffu, nulls);
+#pragma unroll
+	for (int i = 0; i < TOPN_MAXKEYS; i++)
+		if (i < p.nkeys)
+		{
+			for (int o = 16; o > 0; o >>= 1)
+			{
+				const unsigned long long a = __shfl_xor_sync(0xffffffffu, mn[i], o);
+				const unsigned long long b = __shfl_xor_sync(0xffffffffu, mx[i], o);
+
+				mn[i] = a < mn[i] ? a : mn[i];
+				mx[i] = b > mx[i] ? b : mx[i];
+			}
+			if ((threadIdx.x & 31) == 0)
+			{
+				atomicMin(red + i, mn[i]);
+				atomicMax(red + TOPN_MAXKEYS + i, mx[i]);
+				if ((nulls >> i) & 1)
+					atomicOr(red + 2 * TOPN_MAXKEYS + i, 1ull);
+			}
+		}
+}
+
+/* the rows a count / scatter CTA owns: a contiguous chunk of the *nrows input positions */
+__device__ __forceinline__ void
+tsel_chunk(const unsigned long long *nrows, int64_t *lo, int64_t *hi)
+{
+	const int64_t n = (int64_t) *nrows;
+	const int64_t chunk = (n + gridDim.x - 1) / gridDim.x;
+
+	*lo = (int64_t) blockIdx.x * chunk < n ? (int64_t) blockIdx.x * chunk : n;
+	*hi = *lo + chunk < n ? *lo + chunk : n;
+}
+
+/* cnt[CTA][digit]: how many of the CTA's rows have each digit; in = NULL reads rows 0 .. n-1.  st: a selection pass */
+__global__ void __launch_bounds__(TSEL_THREADS)
+k_tsel_count(TselKey k, int shift, const uint32_t *in, const unsigned long long *nrows, const TselState *st, uint32_t *cnt)
+{
+	__shared__ uint32_t h[256];
+	int64_t		lo,
+				hi;
+
+	if (st && st->decided >= 0)
+		return;
+	h[threadIdx.x] = 0;
+	__syncthreads();
+	tsel_chunk(nrows, &lo, &hi);
+	for (int64_t i0 = lo; i0 < hi; i0 += blockDim.x)
+	{
+		const int64_t i = i0 + threadIdx.x;
+		const int	d = i < hi ? tsel_digit(k, shift, in ? in[i] : (uint32_t) i) : -1;
+		/* one shared-memory atomic per digit and warp: a tied key puts every row on the same counter */
+		const unsigned peers = __match_any_sync(0xffffffffu, d);
+
+		if (d >= 0 && (int) (threadIdx.x & 31) == __ffs(peers) - 1)
+			atomicAdd(h + d, (uint32_t) __popc(peers));
+	}
+	__syncthreads();
+	cnt[(int64_t) blockIdx.x * 256 + threadIdx.x] = h[threadIdx.x];
+}
+
+/* one CTA, one thread per digit value: where each (CTA, digit) run of rows goes (off).  Sorting: after every row of a smaller
+ * digit.  Selecting (st): the digit b where the remaining rank falls; rows of smaller digits are chosen (after those chosen
+ * before), rows of digit b are the next tied set - or chosen too when the rank ends with them, which decides the selection */
+__global__ void __launch_bounds__(256)
+k_tsel_plan(const uint32_t *cnt, int grid, TselState *st, int pass, uint32_t *off)
+{
+	__shared__ unsigned long long cum[257];	/* cum[d]: rows with a smaller digit */
+	__shared__ int chosen;
+	const int	d = threadIdx.x;
+	unsigned long long tot = 0,
+				base;
+
+	if (st && st->decided >= 0)
+		return;
+	for (int c = 0; c < grid; c++)
+		tot += cnt[(int64_t) c * 256 + d];
+	cum[d + 1] = tot;
+	if (d == 0)
+		cum[0] = 0;
+	__syncthreads();
+	for (int s = 1; s < 256; s <<= 1)
+	{
+		const unsigned long long add = d + 1 > s ? cum[d + 1 - s] : 0;
+
+		__syncthreads();
+		cum[d + 1] += add;
+		__syncthreads();
+	}
+	base = cum[d];
+	if (st)
+	{
+		const unsigned long long need = st->need;
+
+		if (cum[d] < need && need <= cum[d + 1])
+			chosen = d;
+		__syncthreads();
+		const int	b = chosen;
+		const bool	take = cum[b + 1] == need;
+
+		base = (d < b || (d == b && take)) ? st->nsel + cum[d] : 0;
+		__syncthreads();	/* every thread has read st */
+		if (d == 0)
+		{
+			st->bucket[pass] = b;
+			st->take[pass] = take;
+			st->nsel += take ? cum[b + 1] : cum[b];
+			st->need = take ? 0 : need - cum[b];
+			st->ntied[pass + 1] = take ? 0 : cum[b + 1] - cum[b];
+			if (take)
+				st->decided = pass;
+		}
+	}
+	for (int c = 0; c < grid; c++)
+	{
+		off[(int64_t) c * 256 + d] = (uint32_t) base;
+		base += cnt[(int64_t) c * 256 + d];
+	}
+}
+
+/* each row to off[CTA][digit] plus its rank among the CTA's earlier rows of that digit: the rows of a tile by warp, the rows
+ * of a warp by lane.  Sorting: every row to out.  Selecting (st): digits below the chosen one to out, the chosen one to
+ * out_eq (or out when it completes the selection), larger digits nowhere */
+__global__ void __launch_bounds__(TSEL_THREADS)
+k_tsel_scatter(TselKey k, int shift, const uint32_t *in, const unsigned long long *nrows, const TselState *st, int pass,
+			   const uint32_t *off, uint32_t *out, uint32_t *out_eq)
+{
+	__shared__ uint32_t cur[256];
+	__shared__ uint32_t wpos[TSEL_THREADS / 32][256];	/* rows per (warp, digit) of a tile, then where each warp's run starts */
+	const int	lane = threadIdx.x & 31,
+				warp = threadIdx.x >> 5;
+	int			b = 256,
+				take = 1;
+	int64_t		lo,
+				hi;
+
+	if (st && st->decided >= 0 && st->decided < pass)
+		return;
+	if (st)
+	{
+		b = st->bucket[pass];
+		take = st->take[pass];
+	}
+	cur[threadIdx.x] = off[(int64_t) blockIdx.x * 256 + threadIdx.x];
+	tsel_chunk(nrows, &lo, &hi);
+	for (int64_t i0 = lo; i0 < hi; i0 += blockDim.x)
+	{
+		const int64_t i = i0 + threadIdx.x;
+		const uint32_t row = i < hi ? (in ? in[i] : (uint32_t) i) : 0;
+		const int	d = i < hi ? tsel_digit(k, shift, row) : -1;
+		const unsigned peers = __match_any_sync(0xffffffffu, d);
+
+		for (int w = 0; w < TSEL_THREADS / 32; w++)
+			wpos[w][threadIdx.x] = 0;
+		__syncthreads();
+		if (d >= 0 && lane == __ffs(peers) - 1)
+			wpos[warp][d] = (uint32_t) __popc(peers);
+		__syncthreads();
+		{
+			uint32_t	run = cur[threadIdx.x];
+
+			for (int w = 0; w < TSEL_THREADS / 32; w++)
+			{
+				const uint32_t c = wpos[w][threadIdx.x];
+
+				wpos[w][threadIdx.x] = run;
+				run += c;
+			}
+			cur[threadIdx.x] = run;
+		}
+		__syncthreads();
+		if (d >= 0 && d <= b)
+		{
+			const uint32_t at = wpos[warp][d] + (uint32_t) __popc(peers & ((1u << lane) - 1));
+
+			if (d < b || take)
+				out[at] = row;
+			else
+				out_eq[at] = row;
+		}
+		__syncthreads();
+	}
+}
+
+/* a selection no digit decided: the tied set's first rows (row order) complete it; tied = NULL: rows 0 .. */
+__global__ void
+k_tsel_finish(const uint32_t *tied, const TselState *st, uint32_t *sel)
+{
+	if (st->decided >= 0)
+		return;
+	const int64_t need = (int64_t) st->need;
+	const int64_t at = (int64_t) st->nsel;
+
+	for (int64_t i = (int64_t) blockIdx.x * blockDim.x + threadIdx.x; i < need; i += (int64_t) gridDim.x * blockDim.x)
+		sel[at + i] = tied ? tied[i] : (uint32_t) i;
+}
+
+extern "C" int
+cbgpu_topn_select(cbgpu_ctx *ctx, cbgpu_rel *rel, const cbgpu_sort_key *keys, int32_t nkeys, int64_t limit, uint32_t *host_idx,
+				  int64_t *nout)
+{
+	TselState	hst;				/* before mem: its copy to the device may still be queued when mem drains the stream */
+	unsigned long long red[3 * TOPN_MAXKEYS];
+	CbCallMem	mem(ctx);
+	TselKeys	p;
+	int			dshift[TSEL_MAXDIGITS],
+				dkey[TSEL_MAXDIGITS],
+				nd = 0;
+	unsigned long long *dred = NULL;
+	TselState  *st = NULL;
+	uint32_t   *cnt = NULL,
+			   *sel[2] = {NULL, NULL},
+			   *tied[2] = {NULL, NULL};
+
+	*nout = 0;
+	if (nkeys < 1 || nkeys > TOPN_MAXKEYS)
+		return cb_fail(ctx, CBGPU_ERR_UNSUPPORTED, "device top-N supports 1..4 sort keys (%s%lld keys)", "", nkeys);
+	if (limit < 1)
+		return cb_fail(ctx, CBGPU_ERR_UNSUPPORTED, "device top-N needs LIMIT >= 1 (%sgot %lld)", "", limit);
+	memset(&p, 0, sizeof(p));
+	for (int i = 0; i < nkeys; i++)
+	{
+		const cbgpu_sort_key *k = &keys[i];
+		int			w;
+
+		if (k->col < 0 || k->col >= rel->ncols)
+			return cb_fail(ctx, CBGPU_ERR_INVALID, "cbgpu_topn_select: bad key column%s %lld", "", k->col);
+		w = cb_type_w(rel->types[k->col]);
+		if (w != 1 && w != 4 && w != 8)
+			return cb_fail(ctx, CBGPU_ERR_INVALID, "cbgpu_topn_select: key column%s %lld is not 1, 4 or 8 bytes wide", "", k->col);
+		if (k->float8 && w != 8)
+			return cb_fail(ctx, CBGPU_ERR_INVALID, "cbgpu_topn_select: float8 order over a column narrower than 8 bytes%s (column %lld)", "",
+						   k->col);
+		p.k[i].data = rel->data[k->col];
+		p.k[i].type = rel->types[k->col];
+		p.k[i].desc = k->descending != 0;
+		p.k[i].uns = k->unsigned_cmp != 0;
+		p.k[i].f8 = k->float8 != 0;
+		if (k->nulls == CBGPU_SORT_NULLS_MAP)
+			p.k[i].nullmap = rel->nulls[k->col];
+		else if (k->nulls == CBGPU_SORT_NULLS_COUNT)
+		{
+			if (k->null_col < 0 || k->null_col >= rel->ncols || rel->types[k->null_col] != CB_INT8)
+				return cb_fail(ctx, CBGPU_ERR_INVALID, "cbgpu_topn_select: NULL-source column%s %lld is not an int8 column", "",
+							   k->null_col);
+			p.k[i].ncol = (const long long *) rel->data[k->null_col];
+		}
+		else if (k->nulls != CBGPU_SORT_NULLS_NONE)
+			return cb_fail(ctx, CBGPU_ERR_INVALID, "cbgpu_topn_select: unknown NULL source%s %lld", "", k->nulls);
+	}
+	p.nkeys = nkeys;
+	if (rel->nrows == 0)
+		return CBGPU_OK;
+
+	const int64_t n = rel->nrows;
+	const int64_t m = limit < n ? limit : n;
+	const int	sms = ctx->sm_count > 0 ? ctx->sm_count : 1;
+
+	/* the image pass and its read-back: which digits can vary */
+	CB_CUDA(ctx, mem.alloc(&dred, sizeof(red)));
+	CB_CUDA(ctx, cudaMemsetAsync(dred, 0xFF, TOPN_MAXKEYS * sizeof(unsigned long long), ctx->stream));
+	CB_CUDA(ctx, cudaMemsetAsync(dred + TOPN_MAXKEYS, 0, 2 * TOPN_MAXKEYS * sizeof(unsigned long long), ctx->stream));
+	{
+		const int64_t want = (n + TSEL_THREADS - 1) / TSEL_THREADS;
+		const int	blocks = (int) (want < (int64_t) sms * 8 ? want : (int64_t) sms * 8);
+
+		k_tsel_image<<<blocks, TSEL_THREADS, 0, ctx->stream>>>(p, n, dred);
+		CB_LAUNCHED(ctx, "k_tsel_image");
+	}
+	CB_CUDA(ctx, cudaMemcpyAsync(red, dred, sizeof(red), cudaMemcpyDeviceToHost, ctx->stream));
+	CB_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+	CB_CUDA(ctx, mem.free(dred));
+	for (int i = 0; i < nkeys; i++)
+	{
+		const unsigned long long mn = red[i],
+					mx = red[TOPN_MAXKEYS + i];
+		const bool	values = mn <= mx;
+
+		if (values && red[2 * TOPN_MAXKEYS + i])
+		{
+			dkey[nd] = i;
+			dshift[nd++] = TSEL_NULLDIGIT;
+		}
+		if (values && mn != mx)
+			for (int b = (63 - __builtin_clzll(mn ^ mx)) / 8; b >= 0; b--)
+			{
+				dkey[nd] = i;
+				dshift[nd++] = 8 * b;
+			}
+	}
+
+	/* counts and offsets of one pass: grid CTAs x 256 digits each */
+	const int64_t rows_max = m < n ? n : m;
+	int64_t		want = (rows_max + TSEL_THREADS - 1) / TSEL_THREADS;
+	const int	grid_sel = (int) (want < (int64_t) sms * 4 ? want : (int64_t) sms * 4);
+	const int	npass = m < n ? nd : 0;		/* a LIMIT that takes every row selects nothing */
+
+	want = (m + TSEL_THREADS - 1) / TSEL_THREADS;
+	const int	grid_sort = (int) (want < (int64_t) sms * 4 ? want : (int64_t) sms * 4);
+
+	memset(&hst, 0, sizeof(hst));
+	hst.need = (unsigned long long) m;
+	hst.m = (unsigned long long) m;
+	hst.ntied[0] = (unsigned long long) n;
+	hst.decided = -1;
+	CB_CUDA(ctx, mem.alloc(&st, sizeof(TselState)));
+	CB_CUDA(ctx, mem.copy_in(st, &hst, sizeof(hst)));
+	CB_CUDA(ctx, mem.alloc(&sel[0], (size_t) m * sizeof(uint32_t)));
+	if (nd > 0)
+		CB_CUDA(ctx, mem.alloc(&cnt, (size_t) 2 * 256 * (grid_sel > grid_sort ? grid_sel : grid_sort) * sizeof(uint32_t)));
+	for (int t = 0; t < (npass < 2 ? npass : 2); t++)
+		CB_CUDA(ctx, mem.alloc(&tied[t], (size_t) n * sizeof(uint32_t)));
+
+	/* MSD radix select, most significant digit first */
+	uint32_t   *const off = cnt ? cnt + (size_t) 256 * (grid_sel > grid_sort ? grid_sel : grid_sort) : NULL;
+
+	for (int d = 0; d < npass; d++)
+	{
+		const TselKey k = p.k[dkey[d]];
+		const uint32_t *in = d == 0 ? NULL : tied[(d - 1) & 1];
+
+		k_tsel_count<<<grid_sel, TSEL_THREADS, 0, ctx->stream>>>(k, dshift[d], in, st->ntied + d, st, cnt);
+		CB_LAUNCHED(ctx, "k_tsel_count");
+		k_tsel_plan<<<1, 256, 0, ctx->stream>>>(cnt, grid_sel, st, d, off);
+		CB_LAUNCHED(ctx, "k_tsel_plan");
+		k_tsel_scatter<<<grid_sel, TSEL_THREADS, 0, ctx->stream>>>(k, dshift[d], in, st->ntied + d, st, d, off, sel[0], tied[d & 1]);
+		CB_LAUNCHED(ctx, "k_tsel_scatter");
+	}
+	{
+		const int64_t want_f = (m + TSEL_THREADS - 1) / TSEL_THREADS;
+		const int	blocks = (int) (want_f < (int64_t) sms * 4 ? want_f : (int64_t) sms * 4);
+
+		k_tsel_finish<<<blocks, TSEL_THREADS, 0, ctx->stream>>>(npass == 0 ? NULL : tied[(npass - 1) & 1], st, sel[0]);
+		CB_LAUNCHED(ctx, "k_tsel_finish");
+	}
+	for (int t = 0; t < 2; t++)
+		if (tied[t])
+			CB_CUDA(ctx, mem.free(tied[t]));
+
+	/* stable LSD radix sort of the chosen rows, least significant digit first */
+	int			cur = 0;
+
+	if (nd > 0)
+		CB_CUDA(ctx, mem.alloc(&sel[1], (size_t) m * sizeof(uint32_t)));
+	for (int d = nd - 1; d >= 0; d--)
+	{
+		const TselKey k = p.k[dkey[d]];
+
+		k_tsel_count<<<grid_sort, TSEL_THREADS, 0, ctx->stream>>>(k, dshift[d], sel[cur], &st->m, NULL, cnt);
+		CB_LAUNCHED(ctx, "k_tsel_count");
+		k_tsel_plan<<<1, 256, 0, ctx->stream>>>(cnt, grid_sort, NULL, 0, off);
+		CB_LAUNCHED(ctx, "k_tsel_plan");
+		k_tsel_scatter<<<grid_sort, TSEL_THREADS, 0, ctx->stream>>>(k, dshift[d], sel[cur], &st->m, NULL, 0, off, sel[cur ^ 1], NULL);
+		CB_LAUNCHED(ctx, "k_tsel_scatter");
+		cur ^= 1;
+	}
+	CB_CUDA(ctx, cudaMemcpyAsync(host_idx, sel[cur], (size_t) m * sizeof(uint32_t), cudaMemcpyDeviceToHost, ctx->stream));
+	CB_CUDA(ctx, mem.sync());
+	*nout = m;
+	return CBGPU_OK;
+}

@@ -90,6 +90,7 @@ typedef struct PExpr
 	int			aggfn;			/* CbAggFn that produced it                                          */
 	int			final;			/* finalise when drained (SIMPLE / FINAL agg output)                 */
 	int			argtype;		/* input type of the aggregate                                       */
+	int			argnull;		/* PE_STATE: the argument may be NULL, so N may be 0 (a NULL sum / min / max) */
 	int			restype;
 } PExpr;
 
@@ -1119,8 +1120,8 @@ static int	node_open_inner(CbPlanState *ps, CbStream **out);
 static const char *node_name(CbNodeTag t);
 static int	cluster_run_motion(CbPlanState *ps);
 static int	open_limitsort(CbPlanState *ps, CbStream **out);
-static int	sort_key_columns(CbEState *es, const PExpr *shape, int nshape, int lead, const CbSortKey *keys, int nkeys, int32_t *keycols,
-							 int32_t *desc, int32_t *uns, int *nk_out);
+static int	sort_key_columns(CbEState *es, const PExpr *shape, int nshape, int lead, const CbSortKey *keys, int nkeys, cbgpu_rel *rel,
+							 int topn, cbgpu_sort_key *sk, int *nk_out);
 
 static int
 open_seqscan(CbPlanState *ps, CbStream **out)
@@ -1559,6 +1560,7 @@ typedef struct AccMeta
 	int			nargs;
 	int			dscale;
 	int			argtype;
+	int			argnull;		/* the argument may be NULL                                          */
 } AccMeta;
 
 typedef struct AggPlanInfo
@@ -1602,6 +1604,7 @@ agg_add_aggref(CbEState *es, VarCtx *vcp, CbStream *s, const CbAgg *agg, AggPlan
 		m.state_kind = st->acckind;
 		m.dscale = st->dscale;
 		m.argtype = st->argtype;
+		m.argnull = st->argnull;
 		switch (st->acckind)
 		{
 			case CBP_ACC_COUNT:
@@ -1642,6 +1645,7 @@ agg_add_aggref(CbEState *es, VarCtx *vcp, CbStream *s, const CbAgg *agg, AggPlan
 				return es_fail(es, CBGPU_ERR_INVALID, "aggregate argument is a transition state");
 			m.argtype = s->pe[a].type;
 			m.dscale = s->pe[a].dscale;
+			m.argnull = s->pe[a].maybe_null;
 		}
 		switch (te->op)
 		{
@@ -2096,6 +2100,7 @@ fill_state_pe(PExpr *e, const CbAgg *agg, const CbExpr *aggref, const AccMeta *m
 	e->acckind = m->state_kind;
 	e->aggfn = aggref->op;
 	e->argtype = m->argtype;
+	e->argnull = m->argnull;
 	e->final = agg->aggsplit != CB_AGGSPLIT_INITIAL_SERIAL;
 	e->l = e->r = -1;
 }
@@ -2835,9 +2840,10 @@ motion_recv_stream(CbPlanState *ps, cbgpu_rel *recv, CbStream **out)
 	{
 		/* merge receive (execMotionSortedReceiver, nodeMotion.c:433): the senders' sorted streams lie one after another
 		 * in the receive buffer; read them in merged order */
-		int32_t		keycols[8],
-					desc[8],
-					uns[8];
+		cbgpu_sort_key sk[4];
+		int32_t		keycols[4],
+					desc[4],
+					uns[4];
 		int			nk = 0;
 		int32_t		nruns = 0;
 		uint32_t   *order = NULL;
@@ -2845,7 +2851,13 @@ motion_recv_stream(CbPlanState *ps, cbgpu_rel *recv, CbStream **out)
 
 		if (m->motionType != CB_MOTIONTYPE_GATHER && m->motionType != CB_MOTIONTYPE_GATHER_SINGLE)
 			return es_fail(es, CBGPU_ERR_UNSUPPORTED, "a sorted Motion that is not a Gather");
-		TRY(sort_key_columns(es, p->send_pe, p->send_nout, lead, m->sortkeys, m->nsortkeys, keycols, desc, uns, &nk));
+		TRY(sort_key_columns(es, p->send_pe, p->send_nout, lead, m->sortkeys, m->nsortkeys, recv, 0, sk, &nk));
+		for (int k = 0; k < nk; k++)
+		{
+			keycols[k] = sk[k].col;
+			desc[k] = sk[k].descending;
+			uns[k] = sk[k].unsigned_cmp;
+		}
 		GPU(es, cbgpu_merge_sorted_runs(es->es_ctx, recv, keycols, desc, uns, nk, es->es_numsegments, &order, &nruns));
 		ps->instrument.kernels += cbgpu_kernel_launches(es->es_ctx) - before;
 		if (order)
@@ -3145,53 +3157,88 @@ rel_to_result(CbEState *es, cbgpu_rel *rel, const PExpr *shape, int nshape, cons
 	return CBGPU_OK;
 }
 
-/* sort keys over a materialised stream (columns laid out as stream_materialize / the Motion receive buffer does: one
- * column per scalar, N / lo / hi per transition state, `lead` leading extra columns) -> the device comparators' key columns.
- * Exact 128-bit sums order through (hi signed, lo unsigned). */
+/* sort keys over a materialised stream `rel` (columns laid out as stream_materialize / the Motion receive buffer does: one
+ * column per scalar, N / lo / hi per transition state, `lead` leading extra columns) -> the device comparators' keys.  Exact
+ * 128-bit sums order through (hi signed, lo unsigned).  `topn`: keys for cbgpu_topn_select too - min / max (the value in lo:
+ * an integer, or for float8 the CBP_F8ORD image, whose signed order is float8's) and float8 sums (lo holds the bits); a sum /
+ * min / max over a nullable argument is NULL where its N is 0.  Without it (the merge receive) those stay refused. */
 static int
-sort_key_columns(CbEState *es, const PExpr *shape, int nshape, int lead, const CbSortKey *keys, int nkeys, int32_t *keycols,
-				 int32_t *desc, int32_t *uns, int *nk_out)
+sort_key_columns(CbEState *es, const PExpr *shape, int nshape, int lead, const CbSortKey *keys, int nkeys, cbgpu_rel *rel, int topn,
+				 cbgpu_sort_key *sk, int *nk_out)
 {
 	int			colstart[MAX_OUT];
 	int			nk = 0;
 
 	shape_columns(shape, nshape, lead, colstart);
+	memset(sk, 0, sizeof(cbgpu_sort_key) * 4);
 	for (int k = 0; k < nkeys; k++)
 	{
-		int			att = keys[k].attno;
+		const int	att = keys[k].attno;
+		const PExpr *e;
+		int			c;
 
 		if (att < 1 || att > nshape)
 			return es_fail(es, CBGPU_ERR_INVALID, "sort key %d out of range", att);
-		if (shape[att - 1].kind == PE_STATE)
+		e = &shape[att - 1];
+		c = colstart[att - 1];
+		if (e->kind == PE_STATE)
 		{
-			/* ORDER BY sum(...): order the exact 128-bit sums through (hi signed, lo unsigned) */
-			if (!(shape[att - 1].aggfn == CB_AGG_SUM && shape[att - 1].acckind == CBP_ACC_SUM_INT) &&
-				shape[att - 1].aggfn != CB_AGG_COUNT && shape[att - 1].aggfn != CB_AGG_COUNT_STAR)
+			const int	count = e->aggfn == CB_AGG_COUNT || e->aggfn == CB_AGG_COUNT_STAR;
+			const int	isum = e->aggfn == CB_AGG_SUM && e->acckind == CBP_ACC_SUM_INT;
+			const int	wider = topn && ((e->aggfn == CB_AGG_SUM && e->acckind == CBP_ACC_SUM_FLOAT) ||
+										 e->aggfn == CB_AGG_MIN || e->aggfn == CB_AGG_MAX);
+
+			if (!count && !isum && !wider)
 				return es_fail(es, CBGPU_ERR_UNSUPPORTED, "ORDER BY over this aggregate is not implemented on the GPU path");
-			if (nk + 2 > 4)
+			if (nk + (isum ? 2 : 1) > 4)
 				return es_fail(es, CBGPU_ERR_UNSUPPORTED, "too many sort keys for the device comparators");
-			if (shape[att - 1].aggfn == CB_AGG_SUM)
+			/* count: N itself; a sum: (hi signed, lo unsigned); min / max / float8 sum: lo */
+			for (int part = 0; part < (isum ? 2 : 1); part++)
 			{
-				keycols[nk] = colstart[att - 1] + 2; desc[nk] = keys[k].descending; uns[nk] = 0; nk++;
-				keycols[nk] = colstart[att - 1] + 1; desc[nk] = keys[k].descending; uns[nk] = 1; nk++;
-			}
-			else
-			{
-				keycols[nk] = colstart[att - 1]; desc[nk] = keys[k].descending; uns[nk] = 0; nk++;
+				sk[nk].col = count ? c : isum && part == 0 ? c + 2 : c + 1;
+				sk[nk].descending = keys[k].descending;
+				sk[nk].unsigned_cmp = isum && part == 1;
+				sk[nk].float8 = e->acckind == CBP_ACC_SUM_FLOAT;
+				if (!count && e->argnull)
+				{
+					sk[nk].nulls = CBGPU_SORT_NULLS_COUNT;
+					sk[nk].null_col = c;
+				}
+				nk++;
 			}
 		}
 		else
 		{
 			if (nk + 1 > 4)
 				return es_fail(es, CBGPU_ERR_UNSUPPORTED, "too many sort keys for the device comparators");
-			keycols[nk] = colstart[att - 1]; desc[nk] = keys[k].descending; uns[nk] = 0; nk++;
+			sk[nk].col = c;
+			sk[nk].descending = keys[k].descending;
+			sk[nk].float8 = e->type == CB_FLOAT8;
+			if (e->maybe_null || cbgpu_rel_has_nulls(rel, c))
+				sk[nk].nulls = CBGPU_SORT_NULLS_MAP;
+			nk++;
 		}
 	}
 	*nk_out = nk;
 	return CBGPU_OK;
 }
 
-/* Limit <- Sort: device top-N over the child's materialised rows */
+/* the sorted rows idx[0 .. n) of rel into out: one gather kernel for all rows and columns (row-by-row copies were 60 tiny
+ * memcpys for Q3's ten rows) */
+static int
+limitsort_take(CbEState *es, NodePriv *p, cbgpu_rel *rel, const uint32_t *idx, int64_t n, cbgpu_rel *out)
+{
+	void	   *didx;
+
+	GPU(es, cbgpu_dev_alloc(es->es_ctx, sizeof(uint32_t) * (size_t) n, &didx));
+	p->owned.devs[p->owned.ndevs++] = didx;
+	GPU(es, cbgpu_dev_write(es->es_ctx, didx, sizeof(uint32_t) * (size_t) n, idx));
+	GPU(es, cbgpu_rel_take_rows(out, rel, (const uint32_t *) didx, n));
+	return CBGPU_OK;
+}
+
+/* Limit <- Sort: device top-N over the child's materialised rows.  cbgpu_topn where its contract covers the keys (Q3), else
+ * cbgpu_topn_select */
 static int
 limitsort_run(CbPlanState *ps, cbgpu_rel **out_rel, PExpr *out_shape, int *out_nshape)
 {
@@ -3202,12 +3249,11 @@ limitsort_run(CbPlanState *ps, cbgpu_rel **out_rel, PExpr *out_shape, int *out_n
 	cbgpu_rel  *rel = NULL;
 	PExpr		shape[MAX_OUT];
 	int			nshape;
-	int32_t		keycols[8],
-				desc[8],
-				uns[8];
+	cbgpu_sort_key sk[4];
 	int			nk = 0;
-	uint32_t	idx[64];
+	uint32_t   *idx = NULL;
 	int64_t		nout = 0;
+	int			rc = CBGPU_OK;
 
 	TRY(node_open(ps->lefttree, &s));
 	/* the child's rows as a relation */
@@ -3219,28 +3265,51 @@ limitsort_run(CbPlanState *ps, cbgpu_rel **out_rel, PExpr *out_shape, int *out_n
 		if (te->tag != T_CbVar || te->varno != CB_OUTER_VAR || te->varattno != i + 1)
 			return es_fail(es, CBGPU_ERR_UNSUPPORTED, "Limit/Sort must pass its child's columns through unchanged on the GPU path");
 	}
-	TRY(sort_key_columns(es, shape, nshape, 0, ls->keys, ls->nkeys, keycols, desc, uns, &nk));
+	TRY(sort_key_columns(es, shape, nshape, 0, ls->keys, ls->nkeys, rel, 1, sk, &nk));
 	if (ls->limit < 0)
 		return es_fail(es, CBGPU_ERR_UNSUPPORTED, "Sort without LIMIT is not on the GPU path (nodeSort.c stays on the CPU)");
-	if (ls->limit > 0)
+	if (ls->limit > 0 && cbgpu_rel_nrows(rel) > 0)
 	{
+		const int64_t nrows = cbgpu_rel_nrows(rel);
 		int64_t		before = cbgpu_kernel_launches(es->es_ctx);
+		int			plain = ls->limit <= 64;	/* cbgpu_topn's contract: LIMIT <= 64, no NULL, no float8 */
 
-		GPU(es, cbgpu_topn(es->es_ctx, rel, keycols, desc, uns, nk, ls->limit, idx, &nout));
+		for (int k = 0; k < nk; k++)
+			plain &= sk[k].nulls == CBGPU_SORT_NULLS_NONE && !sk[k].float8;
+		/* cbgpu_topn writes LIMIT entries whatever the row count; cbgpu_topn_select min(LIMIT, rows) */
+		idx = malloc(sizeof(uint32_t) * (size_t) (plain || ls->limit < nrows ? ls->limit : nrows));
+		if (!idx)
+			return es_fail(es, CBGPU_ERR_NOMEM, "out of host memory for %lld sorted row indices", (long long) nrows);
+		if (plain)
+		{
+			int32_t		keycols[4],
+						desc[4],
+						uns[4];
+
+			for (int k = 0; k < nk; k++)
+			{
+				keycols[k] = sk[k].col;
+				desc[k] = sk[k].descending;
+				uns[k] = sk[k].unsigned_cmp;
+			}
+			rc = cbgpu_topn(es->es_ctx, rel, keycols, desc, uns, nk, ls->limit, idx, &nout);
+		}
+		else
+			rc = cbgpu_topn_select(es->es_ctx, rel, sk, nk, ls->limit, idx, &nout);
+		if (rc != CBGPU_OK)
+		{
+			free(idx);
+			return es_fail(es, rc, "%s", cbgpu_last_error(es->es_ctx));
+		}
 		ps->instrument.kernels += cbgpu_kernel_launches(es->es_ctx) - before;
 	}
 	/* the chosen rows, in order, as a small relation of their own */
-	TRY(rel_create_like(es, &p->owned, rel, nout, out_rel));
-	if (nout > 0)
-	{
-		/* one gather kernel for all rows and columns (row-by-row copies were 60 tiny memcpys for Q3's ten rows) */
-		void	   *didx;
-
-		GPU(es, cbgpu_dev_alloc(es->es_ctx, sizeof(uint32_t) * (size_t) nout, &didx));
-		p->owned.devs[p->owned.ndevs++] = didx;
-		GPU(es, cbgpu_dev_write(es->es_ctx, didx, sizeof(uint32_t) * (size_t) nout, idx));
-		GPU(es, cbgpu_rel_take_rows(*out_rel, rel, (const uint32_t *) didx, nout));
-	}
+	rc = rel_create_like(es, &p->owned, rel, nout, out_rel);
+	if (rc == CBGPU_OK && nout > 0)
+		rc = limitsort_take(es, p, rel, idx, nout, *out_rel);
+	free(idx);
+	if (rc != CBGPU_OK)
+		return rc;
 	memcpy(out_shape, shape, sizeof(PExpr) * (size_t) nshape);
 	*out_nshape = nshape;
 	return CBGPU_OK;

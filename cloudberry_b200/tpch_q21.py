@@ -35,8 +35,8 @@ SCHEMA = {
 }
 COMMIT_COL = 29
 SAUDI_ARABIA = tpch.NATIONS.index("SAUDI ARABIA")
-# the device top-N (LimitSort) takes LIMIT <= 64 and refuses Q21's LIMIT 100 (CBGPU_ERR_UNSUPPORTED), so the GPU runs of
-# Q21 ask for the first 64 rows of the same order
+# the LIMIT of the first GPU tests of Q21, written when the device top-N took LIMIT <= 64 only: they ask for the first 64 rows
+# of the query's order.  The device now runs the query's own LIMIT 100 as well (cbgpu_topn_select)
 DEVICE_LIMIT = 64
 
 

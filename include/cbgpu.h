@@ -415,6 +415,30 @@ int			cbgpu_agg_to_rel(cbgpu_aggtable *t, const int32_t *keytypes, cbgpu_rel **o
 int			cbgpu_topn(cbgpu_ctx *ctx, cbgpu_rel *rel, const int32_t *keycols, const int32_t *descending,
 					   const int32_t *unsigned_cmp, int32_t nkeys, int64_t limit, uint32_t *host_idx,
 					   int64_t *nout);
+
+/* where a sort key's NULLs come from */
+typedef enum CbgpuSortNulls
+{
+	CBGPU_SORT_NULLS_NONE = 0,	/* the key is never NULL                                               */
+	CBGPU_SORT_NULLS_MAP,		/* the key column's own NULL map (none: never NULL)                    */
+	CBGPU_SORT_NULLS_COUNT		/* int8 column null_col; 0 means NULL (an aggregate state's N)         */
+} CbgpuSortNulls;
+
+typedef struct cbgpu_sort_key
+{
+	int32_t		col;
+	int32_t		descending;
+	int32_t		unsigned_cmp;	/* compare the widened 64 bits as unsigned                             */
+	int32_t		float8;			/* compare the 8 bytes as float8 (float8_cmp_internal: NaN above all, -0 = +0) */
+	int32_t		nulls;			/* CbgpuSortNulls: NULLs sort last ascending, first descending         */
+	int32_t		null_col;
+} cbgpu_sort_key;
+
+/* device top-N for any LIMIT >= 1 over 1..4 keys that may be NULL or float8: host_idx (room for min(limit, rows)) gets the row
+ * indices of the first min(limit, rows) rows in order, equal keys in row order; *nout their number.  Two host synchronisations
+ * whatever the size; cbgpu_topn stays the call for LIMIT <= 64 over integer keys without NULLs. */
+int			cbgpu_topn_select(cbgpu_ctx *ctx, cbgpu_rel *rel, const cbgpu_sort_key *keys, int32_t nkeys, int64_t limit,
+							  uint32_t *host_idx, int64_t *nout);
 /* Merge receive of a sorted Gather Motion (Motion.sendSorted; execMotionSortedReceiver nodeMotion.c:433, CdbMergeComparator
  * :1010): `rel` holds the senders' sorted streams one after another; *order_dev (device, cbgpu_dev_free; NULL when the
  * arrival order already is the order) lists its rows in merged order - equal keys: the earlier sender first.  NULLs sort
