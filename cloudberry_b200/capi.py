@@ -295,7 +295,8 @@ class CbTupleTableSlot(C.Structure):
 
 class CbInstrumentation(C.Structure):
     _fields_ = [("ntuples", C.c_double), ("nloops", C.c_double), ("kernels", C.c_int64), ("device_ms", C.c_double),
-                ("rows_in", C.c_int64), ("motion_repartitions", C.c_int64), ("hashjoin_nbatch", C.c_int64), ("agg_npartitions", C.c_int64)]
+                ("rows_in", C.c_int64), ("motion_repartitions", C.c_int64), ("hashjoin_nbatch", C.c_int64), ("agg_npartitions", C.c_int64),
+                ("having_ms", C.c_double)]
 
 
 class CbPlanState(C.Structure):
@@ -863,7 +864,7 @@ def _collect_instrument(ps, out):
     out[n.plan.contents.plan_node_id] = {"node": n.type, "ntuples": ins.ntuples, "kernels": ins.kernels,
                                          "device_ms": ins.device_ms, "rows_in": ins.rows_in,
                                          "motion_repartitions": ins.motion_repartitions, "hashjoin_nbatch": ins.hashjoin_nbatch,
-                                         "agg_npartitions": ins.agg_npartitions}
+                                         "agg_npartitions": ins.agg_npartitions, "having_ms": ins.having_ms}
     _collect_instrument(n.lefttree, out)
     _collect_instrument(n.righttree, out)
 

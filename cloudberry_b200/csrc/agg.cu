@@ -84,8 +84,10 @@ cbgpu_agg_create(cbgpu_ctx *ctx, int32_t nkeys, int32_t naccs, const int32_t *ac
 	int			rc;
 
 	*out = NULL;
-	if (nkeys < 0 || nkeys > CBP_MAX_KEYS || naccs < 0 || naccs > CBP_MAX_AGGS)
-		return cb_fail(ctx, CBGPU_ERR_UNSUPPORTED, "aggregate with %s%lld keys/accumulators is beyond the GPU path's limits", "", (long long) (nkeys * 100 + naccs));
+	if (nkeys < 0 || nkeys > CBP_MAX_GROUP_KEYS)
+		return cb_fail(ctx, CBGPU_ERR_UNSUPPORTED, "GROUP BY with %s%lld columns is beyond the GPU path's limit (8)", "", nkeys);
+	if (naccs < 0 || naccs > CBP_MAX_AGGS)
+		return cb_fail(ctx, CBGPU_ERR_UNSUPPORTED, "aggregate with %s%lld accumulators is beyond the GPU path's limit (16)", "", naccs);
 	CbOwned<cbgpu_aggtable> t((cbgpu_aggtable *) calloc(1, sizeof(cbgpu_aggtable)), cbgpu_agg_free);
 
 	if (!t)
@@ -380,9 +382,9 @@ cbgpu_agg_read(cbgpu_aggtable *t, int64_t maxgroups, int64_t *keys, uint32_t *ke
 /* groups -> relation: key columns (typed), then per accumulator N, sum.lo, sum.hi (int8 each) */
 struct AggRelOut
 {
-	void	   *key[CBP_MAX_KEYS];
-	uint8_t    *keynulls[CBP_MAX_KEYS];
-	int32_t		keytype[CBP_MAX_KEYS];
+	void	   *key[CBP_MAX_GROUP_KEYS];
+	uint8_t    *keynulls[CBP_MAX_GROUP_KEYS];
+	int32_t		keytype[CBP_MAX_GROUP_KEYS];
 	int64_t    *acc[CBP_MAX_AGGS * 3];
 	int32_t    *counter;
 };
@@ -447,7 +449,7 @@ cbgpu_agg_to_rel(cbgpu_aggtable *t, const int32_t *keytypes, cbgpu_rel **out)
 	CbCallMem	mem(ctx);
 	int64_t		ng;
 	int			rc = cbgpu_agg_ngroups(t, &ng);
-	int32_t		types[CBP_MAX_KEYS + CBP_MAX_AGGS * 3];
+	int32_t		types[CBP_MAX_GROUP_KEYS + CBP_MAX_AGGS * 3];
 	int			ncols = t->d.nkeys + t->d.naccs * 3;
 	cbgpu_rel  *created;
 	AggRelOut	o;

@@ -151,7 +151,7 @@ struct AggSnap
 	int32_t		audit;
 	int32_t		pad[3];
 	uint32_t	keynull[AGG_SNAP_MAXG];
-	int64_t		keys[AGG_SNAP_MAXG][CBP_MAX_KEYS];
+	int64_t		keys[AGG_SNAP_MAXG][CBP_MAX_GROUP_KEYS];
 	int64_t		n[AGG_SNAP_MAXG][CBP_MAX_AGGS];
 	int64_t		lo[AGG_SNAP_MAXG][CBP_MAX_AGGS];
 	int64_t		hi[AGG_SNAP_MAXG][CBP_MAX_AGGS];

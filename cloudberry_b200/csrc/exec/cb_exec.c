@@ -24,6 +24,7 @@
 #include <stdio.h>
 #include <stdlib.h>
 #include <string.h>
+#include <time.h>
 
 #include "../../../include/cb_exec.h"
 #include "../like_match.cuh"		/* like_pattern_check: a malformed pattern is refused while the plan translates */
@@ -1569,7 +1570,7 @@ typedef struct AggPlanInfo
 	AccMeta		acc[CBP_MAX_AGGS];
 	int			acc_of_target[MAX_OUT];	/* -1: grouping column                                       */
 	int			key_of_target[MAX_OUT];
-	int			keys[CBP_MAX_KEYS];		/* PE ids                                                    */
+	int			keys[CBP_MAX_GROUP_KEYS];	/* PE ids                                                    */
 	int			nkeys;
 	/* HAVING: the Aggref nodes of the qual and the accumulators that hold their states */
 #define MAX_HAVING_AGGS 8
@@ -1739,6 +1740,9 @@ agg_run(CbPlanState *ps, AggPlanInfo *info, cbgpu_aggtable **table_out, CbStream
 	VarCtx		vc;
 	int			outer[MAX_OUT];
 
+	/* refused before the child runs: its joins would build their tables first */
+	if (agg->numCols > CBP_MAX_GROUP_KEYS)
+		return es_fail(es, CBGPU_ERR_UNSUPPORTED, "GROUP BY with %d columns is beyond the GPU path's limit (%d)", agg->numCols, CBP_MAX_GROUP_KEYS);
 	TRY(node_open(ps->lefttree, &s));
 	*child_stream = s;
 	memcpy(outer, s->out, sizeof(int) * (size_t) s->nout);
@@ -1748,8 +1752,6 @@ agg_run(CbPlanState *ps, AggPlanInfo *info, cbgpu_aggtable **table_out, CbStream
 	vc.outer = outer;
 	vc.nouter = s->nout;
 	memset(info, 0, sizeof(*info));
-	if (agg->numCols > CBP_MAX_KEYS)
-		return es_fail(es, CBGPU_ERR_UNSUPPORTED, "GROUP BY with %d columns is beyond the GPU path's limit (%d)", agg->numCols, CBP_MAX_KEYS);
 	if (agg->aggstrategy != CB_AGG_HASHED && agg->aggstrategy != CB_AGG_PLAIN)
 		return es_fail(es, CBGPU_ERR_UNSUPPORTED, "only hashed / plain aggregation runs on the GPU path");
 	info->nkeys = agg->numCols;
@@ -1904,7 +1906,7 @@ agg_run(CbPlanState *ps, AggPlanInfo *info, cbgpu_aggtable **table_out, CbStream
 		cbgpu_rel  *pieces[256];
 		int			npieces = 0;
 		int64_t		total = 0;
-		int32_t		keytypes[CBP_MAX_KEYS];
+		int32_t		keytypes[CBP_MAX_GROUP_KEYS];
 		int			rc = CBGPU_OK;
 		int			overflow = 0;
 
@@ -2158,6 +2160,16 @@ agg_result(CbPlanState *ps)
 				rs->vals[o] = keys[g * nk + k];
 				rs->nulls[o] = (keynull[g] >> k) & 1;
 				rs->types[i] = cs->pe[info.keys[k]].type;
+				if (rs->types[i] == CB_NUMERIC && !rs->nulls[o])
+				{
+					CbNumericDatum *nd = &rs->nums[o];
+
+					nd->lo = keys[g * nk + k];
+					nd->hi = nd->lo < 0 ? -1 : 0;
+					nd->dscale = cs->pe[info.keys[k]].dscale;
+					cb_numeric_sum_text(nd->lo, nd->hi, nd->dscale, nd->text, sizeof(nd->text));
+					rs->vals[o] = (int64_t) (intptr_t) nd;
+				}
 			}
 			else
 			{
@@ -2493,7 +2505,7 @@ open_agg(CbPlanState *ps, CbStream **out)
 	CbStream   *cs,
 			   *s;
 	cbgpu_rel  *rel;
-	int32_t		keytypes[CBP_MAX_KEYS];
+	int32_t		keytypes[CBP_MAX_GROUP_KEYS];
 
 	TRY(agg_run(ps, &info, &t, &cs, &rel));
 	for (int k = 0; k < info.nkeys; k++)
@@ -2515,8 +2527,13 @@ open_agg(CbPlanState *ps, CbStream **out)
 		/* HAVING: the stream reads the groups' relation through the selection of the groups that pass */
 		uint32_t   *sel = NULL;
 		int64_t		nsel = 0;
+		struct timespec t0,
+					t1;
 
+		clock_gettime(CLOCK_MONOTONIC, &t0);
 		TRY(having_select(ps, &info, cs, rel, &sel, &nsel));
+		clock_gettime(CLOCK_MONOTONIC, &t1);
+		ps->instrument.having_ms += (t1.tv_sec - t0.tv_sec) * 1e3 + (t1.tv_nsec - t0.tv_nsec) / 1e6;
 		s->pipe.drv_nsrc = 1;
 		s->pipe.drv_idx[0] = sel;
 		s->pipe.nrows = nsel;

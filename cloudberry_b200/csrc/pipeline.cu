@@ -95,6 +95,8 @@ cb_pipeline_to_dev(cbgpu_ctx *ctx, const CbPipeline *p, PipeDev *d, XProg *xp)
 	switch (s->kind)
 	{
 		case CBP_SINK_AGG:
+			if (s->nkeys < 0 || s->nkeys > CBP_MAX_GROUP_KEYS)
+				return cb_fail(ctx, CBGPU_ERR_UNSUPPORTED, "GROUP BY with %s%lld columns is beyond the GPU path's limit (8)", "", s->nkeys);
 			if (!s->agg || s->nkeys != s->agg->d.nkeys || s->naccs != s->agg->d.naccs)
 				return cb_fail(ctx, CBGPU_ERR_INVALID, "pipeline sink: agg table shape mismatch%s", "", 0);
 			ds->agg = s->agg->d;
@@ -103,10 +105,10 @@ cb_pipeline_to_dev(cbgpu_ctx *ctx, const CbPipeline *p, PipeDev *d, XProg *xp)
 			ds->naccs = s->naccs;
 			for (int k = 0; k < s->nkeys; k++)
 			{
-				ds->keytype[k] = s->keytype[k];
+				/* the group hash only places a group in this table (a Motion routes by cdb_route, which refuses numeric keys):
+				 * a numeric key column has one scale, so its scaled int64 identifies the value and hashes as an int8 */
+				ds->keytype[k] = s->keytype[k] == CB_NUMERIC ? CB_INT8 : s->keytype[k];
 				ds->keydict[k] = s->key_dict_hash[k];
-				if (s->keytype[k] == CB_NUMERIC)
-					return cb_fail(ctx, CBGPU_ERR_UNSUPPORTED, "numeric GROUP BY keys (hash_numeric) are not on the GPU path%s", "", 0);
 			}
 			{
 				int			nargs = xp->depth - s->nkeys;

@@ -51,8 +51,8 @@ struct DSink
 	int32_t		kind;
 	AggDev		agg;
 	int32_t		nkeys;
-	int32_t		keytype[CBP_MAX_KEYS];
-	const uint32_t *keydict[CBP_MAX_KEYS];
+	int32_t		keytype[CBP_MAX_GROUP_KEYS];	/* the key's hash function: a numeric key's is int8's            */
+	const uint32_t *keydict[CBP_MAX_GROUP_KEYS];
 	int32_t		naccs;
 	CbpAcc		accs[CBP_MAX_AGGS];
 	SinkOut		out;

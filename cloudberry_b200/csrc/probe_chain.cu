@@ -116,9 +116,9 @@ struct PcParams
 	int32_t		sink_kind;		/* CBP_SINK_AGG, CBP_SINK_MATERIALIZE or CBP_SINK_PARTITION          */
 	AggDev		agg;
 	int32_t		nkeys;
-	PcCol		key[CBP_MAX_KEYS];
-	int32_t		keytype[CBP_MAX_KEYS];
-	const uint32_t *keydict[CBP_MAX_KEYS];
+	PcCol		key[CBP_MAX_GROUP_KEYS];
+	int32_t		keytype[CBP_MAX_GROUP_KEYS];
+	const uint32_t *keydict[CBP_MAX_GROUP_KEYS];
 	int32_t		naccs;
 	int32_t		acc_term[CBP_MAX_AGGS];	/* -1 = count, else index of the value term               */
 	int32_t		nterms;
@@ -358,7 +358,7 @@ __device__ __noinline__ void
 pc_stage_sink(const PcParams &P, PcQ Q, unsigned base, unsigned n, unsigned long long *s_obase, PcPart *part)
 {
 	const SinkOut &O = P.sink;
-	int64_t		kv[CBP_MAX_KEYS];	/* the group or the hash keys of one row */
+	int64_t		kv[CBP_MAX_GROUP_KEYS];	/* the group or the hash keys of one row */
 
 	if (P.sink_kind == CBP_SINK_AGG)
 	{

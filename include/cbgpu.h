@@ -150,7 +150,8 @@ size_t		cbgpu_rel_nbytes(const cbgpu_rel *rel);
 #define CBP_MAX_SRC 8
 #define CBP_MAX_COLS 40
 #define CBP_MAX_OPS 128
-#define CBP_MAX_KEYS 4
+#define CBP_MAX_KEYS 4			/* keys of a probe, a hash table (cbgpu_ht_build) and a PARTITION sink (nhash) */
+#define CBP_MAX_GROUP_KEYS 8	/* GROUP BY columns of an AGG sink and an agg table (cbgpu_agg_create)       */
 #define CBP_MAX_AGGS 16
 #define CBP_MAX_OUT 48
 #define CBP_STACK 48
@@ -245,11 +246,12 @@ typedef struct CbpAcc
 typedef struct CbpSink
 {
 	int32_t		kind;
-	/* AGG */
+	/* AGG: the first nkeys (0 .. CBP_MAX_GROUP_KEYS) stack values are the group key.  A numeric key is hashed as the int8 of
+	 * its scaled value: one key column has one scale, and the group hash only places groups in the table */
 	cbgpu_aggtable *agg;
 	int32_t		nkeys;
-	int32_t		keytype[CBP_MAX_KEYS];
-	const uint32_t *key_dict_hash[CBP_MAX_KEYS];
+	int32_t		keytype[CBP_MAX_GROUP_KEYS];
+	const uint32_t *key_dict_hash[CBP_MAX_GROUP_KEYS];
 	int32_t		naccs;
 	CbpAcc		accs[CBP_MAX_AGGS];
 	/* MATERIALIZE / PARTITION: the top `nout` stack values become one output row */
@@ -387,7 +389,8 @@ int			cbgpu_rel_share_dict_hash(cbgpu_rel *dst, int32_t dcol, const cbgpu_rel *s
 /* ------------------------------------------------------------------------------------------
  * aggregate tables
  * ------------------------------------------------------------------------------------------ */
-/* acc_kinds[a] (CbpAggKind) fixes each accumulator's initial value (MIN / MAX need one) */
+/* acc_kinds[a] (CbpAggKind) fixes each accumulator's initial value (MIN / MAX need one).  0 <= nkeys <= CBP_MAX_GROUP_KEYS
+ * (0: a plain aggregate, one group); more is CBGPU_ERR_UNSUPPORTED before any allocation */
 int			cbgpu_agg_create(cbgpu_ctx *ctx, int32_t nkeys, int32_t naccs, const int32_t *acc_kinds,
 							 int64_t capacity_groups, cbgpu_aggtable **out);
 void		cbgpu_agg_free(cbgpu_aggtable *t);
