@@ -72,7 +72,26 @@ def topn_select(ctx, rel, keys, limit):
 # CbpOpCode
 (CBP_END, CBP_LOAD, CBP_CONST, CBP_ADD, CBP_SUB, CBP_MUL, CBP_FADD, CBP_FSUB, CBP_FMUL, CBP_I2F, CBP_EQ, CBP_NE, CBP_LT, CBP_LE,
  CBP_GT, CBP_GE, CBP_FEQ, CBP_FNE, CBP_FLT, CBP_FLE, CBP_FGT, CBP_FGE, CBP_AND, CBP_OR, CBP_NOT, CBP_FILTER, CBP_PROBE, CBP_DUP,
- CBP_POP, CBP_F8ORD, CBP_INSET) = range(31)
+ CBP_POP, CBP_F8ORD, CBP_INSET, CBP_STATE) = range(32)
+# HAVING programs (cbgpu_having_select): CONST flags, STATE kinds (imm = kind | scale << 8)
+CBH_CONST_F8, CBH_CONST_NULL = 0x10000, 0x20000
+CBH_COUNT, CBH_SUM, CBH_AVG, CBH_MIN, CBH_MAX, CBH_FSUM, CBH_FAVG, CBH_FMIN, CBH_FMAX = range(1, 10)
+
+
+def having_select(ctx, rel, ops, nquals):
+    """cbgpu_having_select over DeviceRelation rel (a groups relation: keys, then N / lo / hi per accumulator): the ascending
+    row ids of the groups every one of the program's nquals booleans keeps, as a uint32 array.  ops: [(code, a, imm)]."""
+    oa = (CbpOp * max(len(ops), 1))(*[CbpOp(code, a, imm) for code, a, imm in ops])
+    dev, nsel = C.c_void_p(), C.c_int64(0)
+    ctx.check(ctx.L.cbgpu_dev_alloc(ctx.h, 4 * max(rel.nrows, 1), C.byref(dev)))
+    try:
+        ctx.check(ctx.L.cbgpu_having_select(ctx.h, rel.h, oa, len(ops), nquals, dev, C.byref(nsel)))
+        ids = np.zeros(max(nsel.value, 1), dtype=np.uint32)
+        if nsel.value:
+            ctx.check(ctx.L.cbgpu_read_u32(ctx.h, dev, nsel.value, ids.ctypes.data))
+        return ids[:nsel.value]
+    finally:
+        ctx.L.cbgpu_dev_free(ctx.h, dev)
 
 
 def join_filter(cols, ops):
@@ -429,6 +448,7 @@ def gpu():
             "cbgpu_topn": (C.c_int, [vp, vp, C.POINTER(i32), C.POINTER(i32), C.POINTER(i32), i32, i64, C.POINTER(C.c_uint32),
                                      C.POINTER(i64)]),
             "cbgpu_topn_select": (C.c_int, [vp, vp, C.POINTER(CbgpuSortKey), i32, i64, C.POINTER(C.c_uint32), C.POINTER(i64)]),
+            "cbgpu_having_select": (C.c_int, [vp, vp, C.POINTER(CbpOp), i32, i32, vp, C.POINTER(i64)]),
             "cbgpu_rel_take_rows": (C.c_int, [vp, vp, vp, i64]),
             "cbgpu_dev_alloc": (C.c_int, [vp, C.c_size_t, C.POINTER(vp)]),
             "cbgpu_dev_write": (C.c_int, [vp, vp, C.c_size_t, vp]),

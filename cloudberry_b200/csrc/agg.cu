@@ -9,6 +9,8 @@
  * nodes/nodes.h:977-1000 AggSplit) and finalised exactly on the host.
  */
 #include "common.cuh"
+#include "having_eval.cuh"
+#include "xmatch.h"
 
 #include <stdlib.h>
 
@@ -1524,5 +1526,191 @@ cbgpu_topn_select(cbgpu_ctx *ctx, cbgpu_rel *rel, const cbgpu_sort_key *keys, in
 	CB_CUDA(ctx, cudaMemcpyAsync(host_idx, sel[cur], (size_t) m * sizeof(uint32_t), cudaMemcpyDeviceToHost, ctx->stream));
 	CB_CUDA(ctx, mem.sync());
 	*nout = m;
+	return CBGPU_OK;
+}
+
+/* ---------------------------------------------------------------------------------------------
+ * HAVING over a groups relation (ExecQual over the finalised aggregates, nodeAgg.c:2460 / 3100): one thread evaluates one
+ * group's program (having_eval.cuh), a warp ballots its verdicts into a bitmap, each CTA counts its tile's survivors; one CTA
+ * scans the counts; the scatter writes each survivor's id at its rank, so the selection comes in ascending group order.
+ * --------------------------------------------------------------------------------------------- */
+#define HV_THREADS 256			/* groups per CTA: one per thread, eight bitmap words per tile */
+#define HV_WORDS (HV_THREADS / 32)
+#define HV_SCAN_THREADS 1024
+
+struct HavingParams
+{
+	HvCols		cols;
+	CbpOp		ops[CBP_MAX_OPS];
+	int32_t		nops;
+	uint32_t	qmask;			/* bit q: qual q must be true                                        */
+	int64_t		ngroups;
+	int64_t		ntiles;
+	uint32_t   *bits;			/* [ntiles * HV_WORDS] verdicts, bit g % 32 of word g / 32            */
+	uint32_t   *cnt;			/* [ntiles] survivors per tile, then their exclusive prefix           */
+	int64_t    *total;
+	uint32_t   *sel;
+	int		   *status;
+};
+
+/* One group per thread: the float8 division of an avg may call the division's slow path, and more than one group per thread
+ * would keep the loop's state live across that call (spilled) */
+__global__ void __launch_bounds__(HV_THREADS)
+k_having_eval(const HavingParams p)
+{
+	__shared__ CbpOp s_ops[CBP_MAX_OPS];
+	__shared__ uint32_t s_cnt[HV_WORDS];
+	const int	lane = threadIdx.x & 31,
+				warp = threadIdx.x >> 5;
+	const int64_t g = (int64_t) blockIdx.x * HV_THREADS + threadIdx.x;
+	bool		keep = false;
+
+	for (int i = threadIdx.x; i < p.nops; i += HV_THREADS)
+		s_ops[i] = p.ops[i];
+	__syncthreads();
+	if (g < p.ngroups)
+	{
+		const uint64_t r = hv_program(s_ops, p.nops, &p.cols, g);
+
+		keep = (r & p.qmask) == p.qmask;
+		if (r & HV_OVERFLOWED)
+			atomicExch(p.status, CBGPU_ERR_OVERFLOW);
+	}
+	const uint32_t w = __ballot_sync(0xFFFFFFFFu, keep);
+
+	if (lane == 0)
+	{
+		p.bits[(int64_t) blockIdx.x * HV_WORDS + warp] = w;
+		s_cnt[warp] = __popc(w);
+	}
+	__syncthreads();
+	if (threadIdx.x == 0)
+	{
+		uint32_t	t = 0;
+
+		for (int i = 0; i < HV_WORDS; i++)
+			t += s_cnt[i];
+		p.cnt[blockIdx.x] = t;
+	}
+}
+
+/* exclusive prefix of the tiles' counts, in place, and their sum to *total: each thread sums a run of consecutive tiles, the
+ * CTA scans the runs' sums, each thread writes its run's prefixes */
+__global__ void __launch_bounds__(HV_SCAN_THREADS)
+k_having_scan(const HavingParams p)
+{
+	__shared__ uint32_t s_warp[HV_SCAN_THREADS / 32];
+	const int	lane = threadIdx.x & 31,
+				warp = threadIdx.x >> 5;
+	const int64_t per = (p.ntiles + HV_SCAN_THREADS - 1) / HV_SCAN_THREADS;
+	const int64_t lo = threadIdx.x * per,
+				hi = lo + per < p.ntiles ? lo + per : p.ntiles;
+	uint32_t	sum = 0,
+				x;
+
+	for (int64_t i = lo; i < hi; i++)
+		sum += p.cnt[i];
+	x = sum;
+	for (int d = 1; d < 32; d <<= 1)
+	{
+		const uint32_t y = __shfl_up_sync(0xFFFFFFFFu, x, d);
+
+		if (lane >= d)
+			x += y;
+	}
+	if (lane == 31)
+		s_warp[warp] = x;
+	__syncthreads();
+	uint32_t	run = x - sum;
+
+	for (int w = 0; w < warp; w++)
+		run += s_warp[w];
+	for (int64_t i = lo; i < hi; i++)
+	{
+		const uint32_t v = p.cnt[i];
+
+		p.cnt[i] = run;
+		run += v;
+	}
+	if (threadIdx.x == HV_SCAN_THREADS - 1)
+		*p.total = run;
+}
+
+__global__ void __launch_bounds__(HV_THREADS)
+k_having_scatter(const HavingParams p)
+{
+	const int	lane = threadIdx.x & 31,
+				warp = threadIdx.x >> 5;
+	const uint32_t *words = p.bits + (int64_t) blockIdx.x * HV_WORDS;
+	const uint32_t w = words[warp];
+	uint32_t	pos = p.cnt[blockIdx.x];
+
+	if (!((w >> lane) & 1))
+		return;
+	for (int i = 0; i < warp; i++)
+		pos += __popc(words[i]);
+	p.sel[pos + __popc(w & ((1u << lane) - 1))] = (uint32_t) ((int64_t) blockIdx.x * HV_THREADS + threadIdx.x);
+}
+
+extern "C" int
+cbgpu_having_select(cbgpu_ctx *ctx, cbgpu_rel *groups, const CbpOp *ops, int32_t nops, int32_t nquals, uint32_t *sel_dev,
+					int64_t *nsel)
+{
+	CbCallMem	mem(ctx);
+	XProg	   *x = (XProg *) cb_scratch(ctx, 0, sizeof(XProg));
+	HavingParams *p = (HavingParams *) cb_scratch(ctx, 1, sizeof(HavingParams));
+	const int64_t ng = groups->nrows;
+	int64_t		total = 0;
+	int			rc;
+
+	*nsel = 0;
+	if (!x || !p)
+		return cb_fail(ctx, CBGPU_ERR_NOMEM, "HAVING: no host memory%s", "", 0);
+	if (!ops || !sel_dev)
+		return cb_fail(ctx, CBGPU_ERR_INVALID, "cbgpu_having_select: no program or no selection buffer%s", "", 0);
+	rc = xm_check_having(ctx, groups->types, groups->ncols, ops, nops, nquals, x);
+	if (rc)
+		return rc;
+	if (ng > (int64_t) UINT32_MAX)
+		return cb_fail(ctx, CBGPU_ERR_UNSUPPORTED, "HAVING over %s%lld groups: row ids are 32 bits", "", ng);
+	if (ng == 0)
+		return CBGPU_OK;
+	for (int i = 0; i < nops; i++)
+	{
+		if (ops[i].code != CBP_LOAD && ops[i].code != CBP_STATE)
+			continue;
+		/* only the columns the program names are read: a key, or an aggregate's N, lo and hi */
+		for (int col = ops[i].a; col <= ops[i].a + (ops[i].code == CBP_STATE ? 2 : 0); col++)
+		{
+			p->cols.data[col] = groups->data[col];
+			p->cols.nulls[col] = groups->nulls[col];
+			p->cols.width[col] = cb_type_w(groups->types[col]);
+		}
+	}
+	memcpy(p->ops, ops, sizeof(CbpOp) * (size_t) nops);
+	p->nops = nops;
+	p->qmask = nquals >= 32 ? 0xFFFFFFFFu : (1u << nquals) - 1;
+	p->ngroups = ng;
+	p->ntiles = (ng + HV_THREADS - 1) / HV_THREADS;
+	p->sel = sel_dev;
+	p->status = ctx->d_status;
+	CB_CUDA(ctx, mem.alloc(&p->bits, sizeof(uint32_t) * (size_t) p->ntiles * HV_WORDS));
+	CB_CUDA(ctx, mem.alloc(&p->cnt, sizeof(uint32_t) * (size_t) p->ntiles));
+	CB_CUDA(ctx, mem.alloc(&p->total, sizeof(int64_t)));
+	k_having_eval<<<(unsigned) p->ntiles, HV_THREADS, 0, ctx->stream>>>(*p);
+	CB_LAUNCHED(ctx, "k_having_eval");
+	k_having_scan<<<1, HV_SCAN_THREADS, 0, ctx->stream>>>(*p);
+	CB_LAUNCHED(ctx, "k_having_scan");
+	k_having_scatter<<<(unsigned) p->ntiles, HV_THREADS, 0, ctx->stream>>>(*p);
+	CB_LAUNCHED(ctx, "k_having_scatter");
+	/* the one read-back: the survivors' count, with the status word (an overflow) alongside */
+	CB_CUDA(ctx, cudaMemcpyAsync(&total, p->total, sizeof(int64_t), cudaMemcpyDeviceToHost, ctx->stream));
+	CB_CUDA(ctx, CB_STATUS_RIDE(ctx));
+	CB_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+	CB_STATUS_FETCHED(ctx);
+	rc = cb_check_status(ctx, "HAVING");
+	if (rc)
+		return rc;
+	*nsel = total;
 	return CBGPU_OK;
 }

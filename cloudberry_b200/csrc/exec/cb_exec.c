@@ -1728,6 +1728,164 @@ agg_collect_having(CbEState *es, VarCtx *vc, CbStream *s, const CbAgg *agg, AggP
 	return CBGPU_OK;
 }
 
+/* ------------------------------------------------------------------------------------------
+ * HAVING (Agg.plan.qual; ExecQual over the finalised aggregates, nodeAgg.c:2460 / 3100): evaluated on the device over the
+ * groups' relation (cbgpu_having_select).  The groups that pass become a selection vector over that relation.
+ * ------------------------------------------------------------------------------------------ */
+static bool
+having_leaf(const CbExpr *e)
+{
+	return e->tag == T_CbVar || e->tag == T_CbConst || e->tag == T_CbAggref;
+}
+
+/* One qual's shape, from node tags, ops and result types alone: compares of grouping columns, constants and aggregates (two
+ * exact or two float8 operands) under AND / OR / NOT.  Counts the aggregates, the program's ops and the booleans its stack
+ * holds at once. */
+static int
+having_shape(CbEState *es, const CbExpr *e, int *naggs, int *nops, int *nbool, int *maxbool)
+{
+	switch (e->tag)
+	{
+		case T_CbBoolExpr:
+			if (e->nargs < 1 || (e->op == CB_NOT_EXPR && e->nargs != 1))
+				return es_fail(es, CBGPU_ERR_INVALID, "HAVING: malformed boolean expression");
+			for (int i = 0; i < e->nargs; i++)
+			{
+				TRY(having_shape(es, e->args[i], naggs, nops, nbool, maxbool));
+				if (i > 0)
+				{
+					(*nops)++;
+					(*nbool)--;
+				}
+			}
+			if (e->op == CB_NOT_EXPR)
+				(*nops)++;
+			return CBGPU_OK;
+		case T_CbOpExpr:
+			if (e->op == CB_OP_ADD || e->op == CB_OP_SUB || e->op == CB_OP_MUL)
+				return es_fail(es, CBGPU_ERR_UNSUPPORTED, "HAVING on the GPU path takes no arithmetic");
+			if (e->op < CB_OP_EQ || e->op > CB_OP_GE || e->nargs != 2)
+				return es_fail(es, CBGPU_ERR_UNSUPPORTED, "HAVING on the GPU path compares numbers only (operator %d)", e->op);
+			for (int i = 0; i < 2; i++)
+			{
+				const CbExpr *x = e->args[i];
+
+				if (x->tag == T_CbOpExpr && (x->op == CB_OP_ADD || x->op == CB_OP_SUB || x->op == CB_OP_MUL))
+					return es_fail(es, CBGPU_ERR_UNSUPPORTED, "HAVING on the GPU path takes no arithmetic");
+				if (!having_leaf(x))
+					return es_fail(es, CBGPU_ERR_UNSUPPORTED, "HAVING on the GPU path compares grouping columns, constants and aggregates");
+				if (x->tag == T_CbConst && x->restype == CB_TEXT)
+					return es_fail(es, CBGPU_ERR_UNSUPPORTED, "HAVING on the GPU path compares no strings");
+				if (x->tag == T_CbVar && (x->restype == CB_DICT8 || x->restype == CB_DICT32))
+					return es_fail(es, CBGPU_ERR_UNSUPPORTED, "HAVING on the GPU path compares no dictionary-coded grouping column");
+				if (x->restype == CB_BOOL || x->restype == CB_TEXT)
+					return es_fail(es, CBGPU_ERR_UNSUPPORTED, "HAVING on the GPU path compares numbers only");
+				if (x->tag == T_CbAggref)
+					(*naggs)++;
+			}
+			if ((e->args[0]->restype == CB_FLOAT8) != (e->args[1]->restype == CB_FLOAT8))
+				return es_fail(es, CBGPU_ERR_UNSUPPORTED, "HAVING on the GPU path compares two exact or two float8 values, not one of each");
+			*nops += 3;
+			if (++(*nbool) > *maxbool)
+				*maxbool = *nbool;
+			return CBGPU_OK;
+		case T_CbScalarArrayOpExpr:
+			return es_fail(es, CBGPU_ERR_UNSUPPORTED, "HAVING on the GPU path takes no IN / ANY / ALL lists");
+		default:
+			return es_fail(es, CBGPU_ERR_UNSUPPORTED, "HAVING on the GPU path takes compares under AND / OR / NOT");
+	}
+}
+
+/* everything cbgpu_having_select does not evaluate is refused here, before the Agg's child opens */
+static int
+having_check(CbEState *es, const CbPlan *plan)
+{
+	int			naggs = 0,
+				nops = 0,
+				nbool = 0,
+				maxbool = 0;
+
+	for (int q = 0; q < plan->nquals; q++)
+		TRY(having_shape(es, plan->qual[q], &naggs, &nops, &nbool, &maxbool));
+	if (naggs > MAX_HAVING_AGGS)
+		return es_fail(es, CBGPU_ERR_UNSUPPORTED, "more than %d aggregates in HAVING", MAX_HAVING_AGGS);
+	if (nops > CBP_MAX_OPS || maxbool > CBH_MAX_DEPTH)
+		return es_fail(es, CBGPU_ERR_UNSUPPORTED, "HAVING of %d ops holding %d booleans is beyond the GPU path's limits (%d, %d)",
+					   nops, maxbool, CBP_MAX_OPS, CBH_MAX_DEPTH);
+	return CBGPU_OK;
+}
+
+static int
+having_op(CbpOp *ops, int *n, int code, int a, int64_t imm)
+{
+	if (*n >= CBP_MAX_OPS)
+		return CBGPU_ERR_UNSUPPORTED;
+	ops[*n].code = code;
+	ops[*n].a = a;
+	ops[*n].imm = imm;
+	(*n)++;
+	return CBGPU_OK;
+}
+
+/* a qual checked by having_shape -> its postfix program over the groups' relation (keys, then N / lo / hi per accumulator) */
+static int
+having_emit(CbPlanState *ps, const AggPlanInfo *info, CbStream *cs, const CbExpr *e, CbpOp *ops, int *n)
+{
+	CbEState   *es = ps->state;
+	const CbAgg *agg = (const CbAgg *) ps->plan;
+
+	switch (e->tag)
+	{
+		case T_CbVar:
+			for (int k = 0; k < agg->numCols; k++)
+				if (e->varno == CB_OUTER_VAR && agg->grpColIdx[k] == e->varattno)
+				{
+					const PExpr *kx = &cs->pe[info->keys[k]];
+
+					if (kx->type == CB_DICT8 || kx->type == CB_DICT32)
+						return es_fail(es, CBGPU_ERR_UNSUPPORTED, "HAVING on the GPU path compares no dictionary-coded grouping column");
+					return having_op(ops, n, CBP_LOAD, k, kx->dscale);
+				}
+			return es_fail(es, CBGPU_ERR_UNSUPPORTED, "HAVING Var %d is not a grouping column", e->varattno);
+		case T_CbConst:
+			return having_op(ops, n, CBP_CONST, (e->restype == CB_FLOAT8 ? CBH_CONST_F8 : e->dscale) |
+							 (e->constisnull ? CBH_CONST_NULL : 0), e->constval);
+		case T_CbAggref:
+			for (int i = 0; i < info->nhaving; i++)
+				if (info->having_ref[i] == e)
+				{
+					const int	a = info->having_acc[i];
+					const AccMeta *m = &info->acc[a];
+					const bool	f8 = m->state_kind == CBP_ACC_SUM_FLOAT || m->argtype == CB_FLOAT8;
+					int			kind;
+
+					switch (e->op)
+					{
+						case CB_AGG_COUNT_STAR: case CB_AGG_COUNT: kind = CBH_COUNT; break;
+						case CB_AGG_SUM: kind = f8 ? CBH_FSUM : CBH_SUM; break;
+						case CB_AGG_AVG: kind = f8 ? CBH_FAVG : CBH_AVG; break;
+						case CB_AGG_MIN: kind = f8 ? CBH_FMIN : CBH_MIN; break;
+						default: kind = f8 ? CBH_FMAX : CBH_MAX; break;
+					}
+					return having_op(ops, n, CBP_STATE, info->nkeys + 3 * a,
+									 kind | (int64_t) (kind == CBH_COUNT || f8 ? 0 : m->dscale) << 8);
+				}
+			return es_fail(es, CBGPU_ERR_INVALID, "HAVING aggregate without an accumulator");
+		case T_CbOpExpr:
+			TRY(having_emit(ps, info, cs, e->args[0], ops, n));
+			TRY(having_emit(ps, info, cs, e->args[1], ops, n));
+			return having_op(ops, n, (e->args[0]->restype == CB_FLOAT8 ? CBP_FEQ : CBP_EQ) + (e->op - CB_OP_EQ), 0, 0);
+		default:				/* T_CbBoolExpr */
+			for (int i = 0; i < e->nargs; i++)
+			{
+				TRY(having_emit(ps, info, cs, e->args[i], ops, n));
+				if (i > 0)
+					TRY(having_op(ops, n, e->op == CB_AND_EXPR ? CBP_AND : CBP_OR, 0, 0));
+			}
+			return e->op == CB_NOT_EXPR ? having_op(ops, n, CBP_NOT, 0, 0) : CBGPU_OK;
+	}
+}
+
 /* the child's rows aggregated: *table_out holds the groups - or, when they did not fit the operator's memory and the
  * aggregation ran in partitions, *parts_out holds them already as a relation (keys, then N / lo / hi per state) */
 static int
@@ -1743,6 +1901,7 @@ agg_run(CbPlanState *ps, AggPlanInfo *info, cbgpu_aggtable **table_out, CbStream
 	/* refused before the child runs: its joins would build their tables first */
 	if (agg->numCols > CBP_MAX_GROUP_KEYS)
 		return es_fail(es, CBGPU_ERR_UNSUPPORTED, "GROUP BY with %d columns is beyond the GPU path's limit (%d)", agg->numCols, CBP_MAX_GROUP_KEYS);
+	TRY(having_check(es, ps->plan));
 	TRY(node_open(ps->lefttree, &s));
 	*child_stream = s;
 	memcpy(outer, s->out, sizeof(int) * (size_t) s->nout);
@@ -2201,298 +2360,6 @@ agg_result(CbPlanState *ps)
 	return CBGPU_OK;
 }
 
-/* ------------------------------------------------------------------------------------------
- * HAVING (Agg.plan.qual; ExecQual over the finalised aggregates, nodeAgg.c:2460 / 3100): evaluated on the host over the
- * groups' exact states - a value is the rational num / (den * 10^scale) - so that `sum(x) > 100.00` or `avg(x) <= y` decide
- * exactly as numeric arithmetic does.  The groups that pass become a selection vector over the groups' relation.
- * ------------------------------------------------------------------------------------------ */
-typedef struct HVal
-{
-	__int128	num;
-	int64_t		den;			/* > 0                                                                */
-	int			scale;
-	int			isnull;
-	int			isbool;			/* num is 0 / 1                                                       */
-} HVal;
-
-typedef struct HCtx
-{
-	CbEState   *es;
-	const CbAgg *agg;
-	const AggPlanInfo *info;
-	CbStream   *cs;				/* the child's stream: types and scales of the grouping columns           */
-	int64_t		g;				/* group (row of the groups' relation)                                */
-	int64_t   **keycol;			/* [nkeys] widened key values                                         */
-	uint8_t   **keynull;
-	int64_t   **st_n, **st_lo, **st_hi;	/* [naccs]                                                  */
-	int			err;
-} HCtx;
-
-static int
-hv_scale_up(__int128 *v, int k)
-{
-	while (k-- > 0)
-		if (__builtin_mul_overflow(*v, (__int128) 10, v))
-			return 0;
-	return 1;
-}
-
-static HVal
-having_eval(HCtx *h, const CbExpr *e)
-{
-	HVal		r;
-
-	memset(&r, 0, sizeof(r));
-	r.den = 1;
-	switch (e->tag)
-	{
-		case T_CbConst:
-			r.isnull = e->constisnull;
-			r.num = e->constval;
-			r.scale = e->dscale;
-			if (e->restype == CB_FLOAT8)
-				h->err = 1;
-			return r;
-		case T_CbVar:
-			for (int k = 0; k < h->agg->numCols; k++)
-				if (e->varno == CB_OUTER_VAR && h->agg->grpColIdx[k] == e->varattno)
-				{
-					r.isnull = h->keynull[k] ? h->keynull[k][h->g] : 0;
-					r.num = h->keycol[k][h->g];
-					r.scale = h->cs->pe[h->info->keys[k]].dscale;
-					if (h->cs->pe[h->info->keys[k]].type == CB_FLOAT8)
-						h->err = 1;
-					return r;
-				}
-			h->err = 1;
-			return r;
-		case T_CbAggref:
-			for (int i = 0; i < h->info->nhaving; i++)
-				if (h->info->having_ref[i] == e)
-				{
-					const int	a = h->info->having_acc[i];
-					const AccMeta *m = &h->info->acc[a];
-					const int64_t n = h->st_n[a][h->g];
-
-					if (m->state_kind == CBP_ACC_SUM_FLOAT)
-					{
-						h->err = 1;		/* float8 aggregates compare inexactly: not decided here */
-						return r;
-					}
-					r.scale = m->dscale;
-					switch (e->op)
-					{
-						case CB_AGG_COUNT_STAR:
-						case CB_AGG_COUNT:
-							r.num = n;
-							r.scale = 0;
-							return r;
-						case CB_AGG_SUM:
-						case CB_AGG_AVG:
-							r.isnull = n == 0;
-							r.num = ((__int128) h->st_hi[a][h->g] << 64) | (unsigned __int128) (uint64_t) h->st_lo[a][h->g];
-							if (e->op == CB_AGG_AVG && n > 0)
-								r.den = n;
-							return r;
-						case CB_AGG_MIN:
-						case CB_AGG_MAX:
-							r.isnull = n == 0;
-							r.num = h->st_lo[a][h->g];
-							return r;
-					}
-				}
-			h->err = 1;
-			return r;
-		case T_CbOpExpr:
-			{
-				HVal		a,
-							b;
-				__int128	L,
-							R;
-				int			c;
-
-				if (e->nargs != 2 || e->op < CB_OP_EQ)
-				{
-					h->err = 1;		/* arithmetic over aggregates in HAVING: not on this path */
-					return r;
-				}
-				a = having_eval(h, e->args[0]);
-				b = having_eval(h, e->args[1]);
-				r.isbool = 1;
-				if (a.isnull || b.isnull)
-				{
-					r.isnull = 1;
-					return r;
-				}
-				/* a.num / (a.den 10^a.scale)  ?  b.num / (b.den 10^b.scale): cross-multiplied, exact or refused */
-				L = a.num;
-				R = b.num;
-				if (__builtin_mul_overflow(L, (__int128) b.den, &L) || __builtin_mul_overflow(R, (__int128) a.den, &R) ||
-					!hv_scale_up(&L, b.scale > a.scale ? b.scale - a.scale : 0) || !hv_scale_up(&R, a.scale > b.scale ? a.scale - b.scale : 0))
-				{
-					h->err = 2;
-					return r;
-				}
-				c = L < R ? -1 : L > R ? 1 : 0;
-				switch (e->op)
-				{
-					case CB_OP_EQ: r.num = c == 0; break;
-					case CB_OP_NE: r.num = c != 0; break;
-					case CB_OP_LT: r.num = c < 0; break;
-					case CB_OP_LE: r.num = c <= 0; break;
-					case CB_OP_GT: r.num = c > 0; break;
-					default: r.num = c >= 0; break;
-				}
-				return r;
-			}
-		case T_CbBoolExpr:
-			{
-				int			anynull = 0;
-
-				r.isbool = 1;
-				if (e->op == CB_NOT_EXPR)
-				{
-					HVal		a = having_eval(h, e->args[0]);
-
-					r.isnull = a.isnull;
-					r.num = !a.num;
-					return r;
-				}
-				/* three-valued AND / OR (ExecEvalBoolAndStep / OrStep, execExprInterp.c) */
-				r.num = e->op == CB_AND_EXPR;
-				for (int i = 0; i < e->nargs; i++)
-				{
-					HVal		a = having_eval(h, e->args[i]);
-
-					if (a.isnull)
-						anynull = 1;
-					else if (e->op == CB_AND_EXPR && !a.num)
-					{
-						r.num = 0;
-						return r;
-					}
-					else if (e->op == CB_OR_EXPR && a.num)
-					{
-						r.num = 1;
-						return r;
-					}
-				}
-				r.isnull = anynull;
-				return r;
-			}
-		default:
-			h->err = 1;
-			return r;
-	}
-}
-
-/* groups relation `rel` (keys, then N / lo / hi per accumulator) -> device selection vector of the groups HAVING keeps */
-static int
-having_select(CbPlanState *ps, const AggPlanInfo *info, CbStream *cs, cbgpu_rel *rel, uint32_t **sel_dev, int64_t *nsel)
-{
-	CbEState   *es = ps->state;
-	NodePriv   *p = np(ps);
-	const CbAgg *agg = (const CbAgg *) ps->plan;
-	const int64_t ng = cbgpu_rel_nrows(rel);
-	HCtx		h;
-	uint32_t   *sel = calloc((size_t) (ng ? ng : 1), sizeof(uint32_t));
-	int64_t		kept = 0;
-	int			rc = CBGPU_OK;
-	const int	nk = info->nkeys,
-				na = info->naccs;
-	void	   *dev = NULL;
-
-	memset(&h, 0, sizeof(h));
-	h.es = es;
-	h.agg = agg;
-	h.info = info;
-	h.cs = cs;
-	h.keycol = calloc((size_t) (nk ? nk : 1), sizeof(int64_t *));
-	h.keynull = calloc((size_t) (nk ? nk : 1), sizeof(uint8_t *));
-	h.st_n = calloc((size_t) (na ? na : 1), sizeof(int64_t *));
-	h.st_lo = calloc((size_t) (na ? na : 1), sizeof(int64_t *));
-	h.st_hi = calloc((size_t) (na ? na : 1), sizeof(int64_t *));
-	for (int k = 0; k < nk && rc == CBGPU_OK; k++)
-	{
-		const int	w = cb_type_width((CbTypeId) cbgpu_rel_col_type(rel, k));
-		char	   *raw = calloc((size_t) (ng ? ng : 1), (size_t) w);
-
-		h.keycol[k] = calloc((size_t) (ng ? ng : 1), sizeof(int64_t));
-		h.keynull[k] = calloc((size_t) (ng ? ng : 1), 1);
-		if (ng > 0)
-			rc = cbgpu_rel_read_column(rel, k, 0, ng, raw, h.keynull[k]);
-		for (int64_t g = 0; g < ng; g++)
-			h.keycol[k][g] = w == 1 ? ((uint8_t *) raw)[g] : w == 4 ? ((int32_t *) raw)[g] : ((int64_t *) raw)[g];
-		free(raw);
-	}
-	for (int i = 0; i < info->nhaving && rc == CBGPU_OK; i++)
-	{
-		const int	a = info->having_acc[i];
-
-		if (h.st_n[a])
-			continue;
-		h.st_n[a] = calloc((size_t) (ng ? ng : 1), sizeof(int64_t));
-		h.st_lo[a] = calloc((size_t) (ng ? ng : 1), sizeof(int64_t));
-		h.st_hi[a] = calloc((size_t) (ng ? ng : 1), sizeof(int64_t));
-		if (ng > 0)
-		{
-			rc = cbgpu_rel_read_column(rel, nk + 3 * a, 0, ng, h.st_n[a], NULL);
-			if (rc == CBGPU_OK)
-				rc = cbgpu_rel_read_column(rel, nk + 3 * a + 1, 0, ng, h.st_lo[a], NULL);
-			if (rc == CBGPU_OK)
-				rc = cbgpu_rel_read_column(rel, nk + 3 * a + 2, 0, ng, h.st_hi[a], NULL);
-		}
-	}
-	for (int64_t g = 0; g < ng && rc == CBGPU_OK && !h.err; g++)
-	{
-		int			keep = 1;
-
-		h.g = g;
-		for (int q = 0; q < ps->plan->nquals && keep; q++)
-		{
-			HVal		v = having_eval(&h, ps->plan->qual[q]);
-
-			keep = !v.isnull && v.num != 0;	/* ExecQual: NULL counts as false */
-		}
-		if (keep)
-			sel[kept++] = (uint32_t) g;
-	}
-	if (rc != CBGPU_OK)
-		rc = es_fail(es, rc, "%s", cbgpu_last_error(es->es_ctx));
-	else if (h.err == 2)
-		rc = es_fail(es, CBGPU_ERR_OVERFLOW, "HAVING: a comparison of aggregates left 128 bits");
-	else if (h.err)
-		rc = es_fail(es, CBGPU_ERR_UNSUPPORTED, "HAVING on the GPU path compares aggregates, grouping columns and constants (no arithmetic, no float8)");
-	if (rc == CBGPU_OK)
-	{
-		rc = cbgpu_dev_alloc(es->es_ctx, sizeof(uint32_t) * (size_t) (kept ? kept : 1), &dev);
-		if (rc == CBGPU_OK)
-		{
-			p->owned.devs[p->owned.ndevs++] = dev;
-			if (kept > 0)
-				rc = cbgpu_dev_write(es->es_ctx, dev, sizeof(uint32_t) * (size_t) kept, sel);
-		}
-		if (rc != CBGPU_OK)
-			rc = es_fail(es, rc, "%s", cbgpu_last_error(es->es_ctx));
-	}
-	for (int k = 0; k < nk; k++)
-	{
-		free(h.keycol[k]);
-		free(h.keynull[k]);
-	}
-	for (int a = 0; a < na; a++)
-	{
-		free(h.st_n[a]);
-		free(h.st_lo[a]);
-		free(h.st_hi[a]);
-	}
-	free(h.keycol); free(h.keynull); free(h.st_n); free(h.st_lo); free(h.st_hi);
-	free(sel);
-	*sel_dev = (uint32_t *) dev;
-	*nsel = kept;
-	return rc;
-}
-
 /* Agg feeding a parent on the device: groups become a relation (keys, then N / lo / hi per state) */
 static int
 open_agg(CbPlanState *ps, CbStream **out)
@@ -2522,20 +2389,27 @@ open_agg(CbPlanState *ps, CbStream **out)
 	s->rows_in = s->pipe.nrows;
 	s->nsrc = 1;
 	s->nout = ps->plan->ntargets;
-	if (ps->plan->nquals > 0)
+	if (ps->plan->nquals > 0 && s->pipe.nrows > 0)
 	{
-		/* HAVING: the stream reads the groups' relation through the selection of the groups that pass */
-		uint32_t   *sel = NULL;
+		/* HAVING: the stream reads the groups' relation through the selection of the groups that pass (over no groups it
+		 * keeps none, and there is nothing to evaluate) */
+		CbpOp		ops[CBP_MAX_OPS];
+		int			nops = 0;
+		void	   *sel = NULL;
 		int64_t		nsel = 0;
 		struct timespec t0,
 					t1;
 
+		for (int q = 0; q < ps->plan->nquals; q++)
+			TRY(having_emit(ps, &info, cs, ps->plan->qual[q], ops, &nops));
+		GPU(es, cbgpu_dev_alloc(es->es_ctx, sizeof(uint32_t) * (size_t) s->pipe.nrows, &sel));
+		p->owned.devs[p->owned.ndevs++] = sel;
 		clock_gettime(CLOCK_MONOTONIC, &t0);
-		TRY(having_select(ps, &info, cs, rel, &sel, &nsel));
+		GPU(es, cbgpu_having_select(es->es_ctx, rel, ops, nops, ps->plan->nquals, (uint32_t *) sel, &nsel));
 		clock_gettime(CLOCK_MONOTONIC, &t1);
 		ps->instrument.having_ms += (t1.tv_sec - t0.tv_sec) * 1e3 + (t1.tv_nsec - t0.tv_nsec) / 1e6;
 		s->pipe.drv_nsrc = 1;
-		s->pipe.drv_idx[0] = sel;
+		s->pipe.drv_idx[0] = (const uint32_t *) sel;
 		s->pipe.nrows = nsel;
 	}
 	for (int i = 0; i < ps->plan->ntargets; i++)

@@ -47,7 +47,7 @@ xm_effect(const CbpOp &op, const CbpProbe *probes)
 {
 	switch (op.code)
 	{
-		case CBP_LOAD: case CBP_CONST: case CBP_DUP: case XOP_MULCSUB:
+		case CBP_LOAD: case CBP_CONST: case CBP_DUP: case CBP_STATE: case XOP_MULCSUB:
 			return {0, 1};
 		case CBP_NOT: case CBP_I2F: case CBP_F8ORD: case CBP_INSET:
 			return {1, 1};
@@ -64,9 +64,12 @@ xm_effect(const CbpOp &op, const CbpProbe *probes)
 
 /* opcodes as bits of XAllow.ops */
 #define XM_OP(c) (1u << (c))
-#define XM_PIPELINE_OPS (XM_OP(CBP_INSET + 1) - 1)	/* every CbpOpCode (INSET is the last) */
+#define XM_PIPELINE_OPS (XM_OP(CBP_INSET + 1) - 1)	/* every CbpOpCode up to INSET (STATE is HAVING's alone) */
 /* join filters: no FILTER / PROBE / END, and no INSET (they take no code sets) */
 #define XM_SCALAR_OPS (XM_PIPELINE_OPS & ~(XM_OP(CBP_FILTER) | XM_OP(CBP_PROBE) | XM_OP(CBP_END) | XM_OP(CBP_INSET)))
+/* HAVING (cbgpu_having_select): leaves, compares and the boolean operators */
+#define XM_HAVING_OPS (XM_OP(CBP_LOAD) | XM_OP(CBP_CONST) | XM_OP(CBP_STATE) | ((XM_OP(CBP_FGE + 1) - 1) & ~(XM_OP(CBP_EQ) - 1)) | \
+					   XM_OP(CBP_AND) | XM_OP(CBP_OR) | XM_OP(CBP_NOT))
 
 /* what a caller lets a program hold, and how it reports a refusal */
 struct XAllow
@@ -228,4 +231,88 @@ xm_qual_range(int code, int64_t v, int64_t dlo, int64_t dhi, int64_t *lo, int64_
 	*lo = l < INT32_MIN ? INT32_MIN : l;
 	*hi = h > INT32_MAX ? INT32_MAX : h;
 	return true;
+}
+
+/* A HAVING program (cbgpu_having_select) over a groups relation whose columns have types[0 .. ncols): xm_walk with the HAVING
+ * opcodes, then operand kinds.  LOAD, CONST and STATE are exact or float8 values, a compare takes two exact operands (EQ..GE)
+ * or two float8 ones (FEQ..FGE) and makes a boolean, AND / OR / NOT take booleans, and the program leaves nquals (>= 1)
+ * booleans.  So every compare's operands are the two leaf ops before it (having_eval.cuh relies on that).  CBGPU_ERR_INVALID
+ * for a malformed program; CBGPU_ERR_UNSUPPORTED for more than CBH_MAX_DEPTH booleans on the stack at once. */
+static inline int
+xm_check_having(cbgpu_ctx *ctx, const int32_t *types, int ncols, const CbpOp *ops, int nops, int nquals, XProg *x)
+{
+	enum { K_EXACT = 1, K_F8, K_BOOL };
+	const XAllow allow = {"HAVING", XM_HAVING_OPS, NULL, 0, CBGPU_ERR_UNSUPPORTED, 0};
+	int			kind[CBP_MAX_OPS];
+	int			nbool = 0;
+
+	if (nops < 1 || nops > CBP_MAX_OPS || nquals < 1)
+		return cb_fail(ctx, CBGPU_ERR_INVALID, "HAVING program of %s%lld ops", "", nops);
+	int			rc = xm_walk(ctx, allow, ncols, ops, nops, x);
+
+	if (rc)
+		return rc;
+	for (int i = 0; i < x->n; i++)
+	{
+		const XNode *nd = &x->nodes[i];
+		const int64_t scale = nd->code == CBP_STATE ? nd->imm >> 8 : nd->code == CBP_LOAD ? nd->imm : nd->a & 0xFFFF;
+
+		switch (nd->code)
+		{
+			case CBP_LOAD:
+				if (types[nd->a] == CB_FLOAT8)
+					kind[i] = K_F8;
+				else if (types[nd->a] == CB_INT4 || types[nd->a] == CB_INT8 || types[nd->a] == CB_DATE ||
+						 types[nd->a] == CB_NUMERIC || types[nd->a] == CB_BPCHAR1)
+					kind[i] = K_EXACT;
+				else
+					return cb_fail(ctx, CBGPU_ERR_INVALID, "HAVING op %s%lld: LOAD of a column that is not a number", "", i);
+				break;
+			case CBP_CONST:
+				if (nd->a & ~(0xFFFF | CBH_CONST_F8 | CBH_CONST_NULL))
+					return cb_fail(ctx, CBGPU_ERR_INVALID, "HAVING op %s%lld: bad CONST flags", "", i);
+				kind[i] = (nd->a & CBH_CONST_F8) ? K_F8 : K_EXACT;
+				break;
+			case CBP_STATE:
+				{
+					const int	k = (int) (nd->imm & 0xFF);
+
+					if (nd->a < 0 || nd->a + 2 >= ncols || types[nd->a] != CB_INT8 || types[nd->a + 1] != CB_INT8 ||
+						types[nd->a + 2] != CB_INT8)
+						return cb_fail(ctx, CBGPU_ERR_INVALID, "HAVING op %s%lld: STATE of columns that are not (N, lo, hi)", "", i);
+					if (k < CBH_COUNT || k > CBH_FMAX || nd->imm < 0)
+						return cb_fail(ctx, CBGPU_ERR_INVALID, "HAVING op %s%lld: unknown aggregate kind", "", i);
+					kind[i] = k >= CBH_FSUM ? K_F8 : K_EXACT;
+					break;
+				}
+			case CBP_AND: case CBP_OR: case CBP_NOT:
+				if (kind[nd->l] != K_BOOL || (nd->code != CBP_NOT && kind[nd->r] != K_BOOL))
+					return cb_fail(ctx, CBGPU_ERR_INVALID, "HAVING op %s%lld: AND / OR / NOT of a value that is not a boolean", "", i);
+				kind[i] = K_BOOL;
+				break;
+			default:			/* the compares */
+				{
+					const int	want = nd->code >= CBP_FEQ ? K_F8 : K_EXACT;
+
+					if (kind[nd->l] != want || kind[nd->r] != want)
+						return cb_fail(ctx, CBGPU_ERR_INVALID, "HAVING op %s%lld: a compare takes two exact or two float8 operands", "", i);
+					kind[i] = K_BOOL;
+					break;
+				}
+		}
+		if (kind[i] != K_BOOL && (scale < 0 || scale > CBH_MAX_SCALE))
+			return cb_fail(ctx, CBGPU_ERR_INVALID, "HAVING op %s%lld: scale out of range", "", i);
+	}
+	if (x->depth != nquals)
+		return cb_fail(ctx, CBGPU_ERR_INVALID, "HAVING program leaves %s%lld values, not one per qual", "", x->depth);
+	for (int q = 0; q < x->depth; q++)
+		if (kind[x->stack[q]] != K_BOOL)
+			return cb_fail(ctx, CBGPU_ERR_INVALID, "HAVING program leaves a value that is not a boolean%s (qual %lld)", "", q);
+	for (int i = 0; i < nops; i++)
+	{
+		nbool += ops[i].code >= CBP_EQ && ops[i].code <= CBP_FGE ? 1 : ops[i].code == CBP_AND || ops[i].code == CBP_OR ? -1 : 0;
+		if (nbool > CBH_MAX_DEPTH)
+			return cb_fail(ctx, CBGPU_ERR_UNSUPPORTED, "HAVING program holds more than %s%lld booleans at once", "", CBH_MAX_DEPTH);
+	}
+	return CBGPU_OK;
 }

@@ -74,8 +74,8 @@ typedef struct CbInstrumentation
 								 * outgrew its share (data skew)                                     */
 	int64_t		hashjoin_nbatch;	/* Hash: batches the build side was split into (1: it fitted)        */
 	int64_t		agg_npartitions;	/* Agg: passes a partitioned aggregation took (1: the table fitted)  */
-	double		having_ms;		/* Agg: host time of HAVING (read the groups' keys and states, select the groups
-								 * that pass, upload the selection)                                  */
+	double		having_ms;		/* Agg: time of the device HAVING step (host clock around cbgpu_having_select's
+								 * launches and its one read-back of the selected count)             */
 } CbInstrumentation;
 
 typedef struct CbPlanState

@@ -174,9 +174,11 @@ typedef enum CbpOpCode
 	CBP_F8ORD,			/* float8 bits -> an int64 whose integer order is float8's (float8_cmp_internal, utils/adt/float.c: every
 						 * NaN equal and above everything); its own inverse on non-NaN values.  Lets min / max(float8) use
 						 * the integer min / max accumulators */
-	CBP_INSET			/* a = code set (CbPipeline.sets); pop a dictionary code, push whether its bit is set: false for a code
+	CBP_INSET,			/* a = code set (CbPipeline.sets); pop a dictionary code, push whether its bit is set: false for a code
 						 * outside [0, nbits), NULL for NULL.  LIKE / NOT LIKE / IN lists over dictionary columns.  Pipelines
 						 * only (not join filters); runs on the generic kernel */
+	CBP_STATE			/* HAVING programs only (cbgpu_having_select): a = the column of an accumulator's N, imm = CbhStateKind |
+						 * scale << 8; push the aggregate's value from its (N, lo, hi) columns */
 } CbpOpCode;
 
 #define CBP_MAX_SETS 4
@@ -411,6 +413,35 @@ int			cbgpu_agg_read(cbgpu_aggtable *t, int64_t maxgroups, int64_t *keys, uint32
  * 128-bit sum as two int8 columns (lo, hi); used as the source of the next pipeline (Motion,
  * final aggregation) and by top-N */
 int			cbgpu_agg_to_rel(cbgpu_aggtable *t, const int32_t *keytypes, cbgpu_rel **out);
+
+/* HAVING programs: postfix CbpOps over a groups relation in cbgpu_agg_to_rel's layout.
+ *   LOAD    a = a grouping column, imm = its numeric scale (a float8 column is a float8 value)
+ *   CONST   imm = the value (float8: its bits), a = its scale | CBH_CONST_F8 | CBH_CONST_NULL
+ *   STATE   a = the column of N (lo and hi follow it), imm = CbhStateKind | scale << 8
+ *   EQ..GE over two exact operands, FEQ..FGE over two float8 operands, AND / OR / NOT over booleans.
+ * An exact value is the rational num / (den * 10^scale) with a 128-bit num, compared exactly by cross-multiplying; a float8
+ * value compares as float8_cmp_internal orders it (NaN equal to NaN and above everything, -0 equal to +0). */
+#define CBH_CONST_F8 0x10000
+#define CBH_CONST_NULL 0x20000
+#define CBH_MAX_SCALE 1000		/* numeric's largest display scale (NUMERIC_MAX_DISPLAY_SCALE)                  */
+#define CBH_MAX_DEPTH 32		/* booleans a HAVING program may hold on its stack at once                        */
+typedef enum CbhStateKind
+{
+	CBH_COUNT = 1,				/* N                                                                  */
+	CBH_SUM,					/* (hi:lo); NULL when N = 0                                           */
+	CBH_AVG,					/* (hi:lo) / N; NULL when N = 0                                       */
+	CBH_MIN, CBH_MAX,			/* lo; NULL when N = 0                                                */
+	CBH_FSUM,					/* float8: the Sx bits in lo; NULL when N = 0                         */
+	CBH_FAVG,					/* float8: Sx / N; NULL when N = 0                                    */
+	CBH_FMIN, CBH_FMAX			/* float8: lo holds the CBP_F8ORD image; NULL when N = 0              */
+} CbhStateKind;
+/* HAVING over a groups relation in cbgpu_agg_to_rel's layout (keys, then N / lo / hi per accumulator): the ascending row ids
+ * of the groups for which every boolean the program leaves is true (ExecQual: NULL is false) go to sel_dev[0 .. *nsel).
+ * sel_dev is the caller's, with room for every group.  CBGPU_ERR_INVALID, before any launch, for a malformed program or one
+ * that does not leave exactly nquals booleans; CBGPU_ERR_UNSUPPORTED for more than CBH_MAX_DEPTH booleans on its stack;
+ * CBGPU_ERR_OVERFLOW when a compare of two non-NULL exact values needs more than 128 bits for a cross-product. */
+int			cbgpu_having_select(cbgpu_ctx *ctx, cbgpu_rel *groups, const CbpOp *ops, int32_t nops, int32_t nquals,
+								uint32_t *sel_dev, int64_t *nsel);
 
 /* device top-N over a relation: ORDER BY up to 4 (column, descending) keys LIMIT n; 128-bit
  * values are ordered through (hi, lo) column pairs: pass hi as the key and lo as the next key.

@@ -1,8 +1,8 @@
 #!/usr/bin/env python3
 """TPC-H Q10 and Q18 (tpch_q10_q18) on one GPU.  Prints one JSON line: the GPU (name, power limit), and per query the wall time
 of each run (host clock around a query that ends in a read-back) with the summed device time of its pipeline kernels
-(instrument device_ms).  For Q18 it also reports the host HAVING step of its IN subquery (instrument having_ms: the host
-reads every group's key and state, selects the groups that pass and uploads the selection), which is part of the wall time.
+(instrument device_ms).  For Q18 it also reports the HAVING step of its IN subquery (instrument having_ms: host clock around
+the device's evaluation of every group and its one read-back of the selected count), which is part of the wall time.
 With --check-sf (default 1) both queries are run once more at that scale factor and their rows compared with the numpy
 answers (result_check).
 
@@ -54,7 +54,7 @@ def main():
         out[name] = {"wall_ms": [round(r[0], 2) for r in runs], "device_ms": [round(r[1], 2) for r in runs],
                      "rows": runs[0][3]}
         if name == "q18":
-            out[name]["having_host_ms"] = [round(r[2], 2) for r in runs]
+            out[name]["having_ms"] = [round(r[2], 2) for r in runs]
     ex.close()
     for d in dev:
         d.free()
